@@ -1,6 +1,7 @@
 """Benchmark of the CFR hot path (BASELINE.json metric: CFR+ iterations/s, beside the CPU path on the same box).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload fhp|leduc_b5|leduc_b3|leduc_pot]
+                    [--dump-outputs DIR]
 
 A "step" = one full CFR+ iteration (both seats: value/regret sweep + reach/average sweep each) over the whole public
 tree, with the exact best-response evaluation of the current AND the average strategy every `--eval-every` iterations
@@ -16,7 +17,8 @@ bottom-up sweep, pokerrl_b200/distributed.py); the Leduc workloads run one indep
 `starting_stack_sizes` axis, weak scaling, no data-path collective).
 
 Rank 0 prints ONE JSON line.  `--impl reference` times the CPU restatement of the reference's path on the host cores
-(/root/reference does not exist on the GPU box): the C oracles (OpenMP, all host threads) - oracle/cfr_oracle.c for Leduc;
+(the reference's own Python code is not part of this repository): the C oracles (OpenMP, all host threads) -
+oracle/cfr_oracle.c for Leduc;
 for fhp, a game the reference cannot run at all (SURVEY.md headline 2), oracle/cfr2_oracle.c (float64, the same O(R)
 showdown algorithm class as the GPU) on the first FHP_CPU_BOARDS board classes, a whole fixed instance that the GPU arm
 also reports as a matched pair; the full-game figure is that instance scaled by the board count (cost is per board).
@@ -39,6 +41,8 @@ for _p in (ROOT, os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests")):
 LEDUC = {"leduc_b5": "B_5", "leduc_b3": "B_3", "leduc_pot": "POT_ONLY"}
 WORKLOADS = ["fhp", "hulh"] + list(LEDUC) + ["env", "handeval"]
 HULH_FLOP = (0, 5, 10)  # 2h 3d 4s
+HBM_PEAK_GBS = 3350.0  # H100 SXM data sheet (HBM3); MEASURED_PEAKS.json, when present, overrides it
+DUMP_BYTES = 60 * 10 ** 6  # --dump-outputs: at most 64 MB in all, npy headers included
 
 
 # ---------------------------------------------------------------------------------------------------------- workloads
@@ -90,27 +94,33 @@ def algorithmic_bytes(st, two_card):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region; the sampler is stopped at exit in any case."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
 
     def __init__(self, gpu_index):
+        import atexit
         self.proc, self.path = None, "/tmp/prl_clocks_%d.csv" % os.getpid()
         try:
             self.f = open(self.path, "w")
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(gpu_index), "--query-gpu=" + self.Q,
                                           "--format=csv,noheader,nounits", "-lms", "50"], stdout=self.f,
                                          stderr=subprocess.DEVNULL)
+            atexit.register(self._kill)
         except Exception:
             self.proc = None
+
+    def _kill(self):
+        if self.proc is not None and self.proc.poll() is None:
+            self.proc.terminate()
+            self.proc.wait()
 
     def stop(self):
         if self.proc is None:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
-        self.proc.terminate()
-        self.proc.wait()
+        self._kill()
         self.f.close()
         sm, smax, power, reasons = [], None, [], set()
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
@@ -130,6 +140,25 @@ class ClockSampler:
         os.unlink(self.path)
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": smax, "reasons": sorted(reasons),
                 "samples": len(sm), "power_w_max": max(power) if power else None}
+
+
+def dump_outputs(path, arrays, tables):
+    """--dump-outputs: `arrays` as they are and a fixed seeded sample of the rows of each large device table in `tables`,
+    as path/<name>.npy in float32 / float64, at most DUMP_BYTES in all."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    out = {}
+    for k, v in arrays.items():
+        v = v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v, np.float64)
+        out[k] = v if v.dtype in (np.float32, np.float64) else v.astype(np.float64)
+    budget = (DUMP_BYTES - sum(v.nbytes for v in out.values())) // max(len(tables), 1)
+    for k, t in tables.items():
+        n = min(int(t.shape[0]), budget // (int(t.shape[1]) * t.element_size()))
+        idx = np.sort(np.random.default_rng(0).choice(int(t.shape[0]), n, replace=False))
+        out[k] = t[torch.from_numpy(idx).to(t.device)].cpu().numpy()
+    for k, v in out.items():
+        np.save(os.path.join(path, k + ".npy"), v)
 
 
 # ---------------------------------------------------------------------------------------------------------- CPU arms
@@ -228,14 +257,14 @@ def run_aux(a):
     import numpy as np
     import torch
     torch.cuda.set_device(0)
-    K = a.steps or 200
-    W = max(3, a.warmup or 5)
+    K = a.steps if a.steps is not None else 200
+    W = max(3, a.warmup if a.warmup is not None else 5)
     peaks = {}
     try:
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", HBM_PEAK_GBS))
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     sampler = ClockSampler(0)
     time.sleep(0.3)
@@ -414,6 +443,7 @@ def main_fhp(a, rank, world, local_rank):
             "e2e": {"value": v, "unit": "iterations/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}))
         return
 
+    import numpy as np
     import torch
     import torch.distributed as dist
     from pokerrl_b200 import _native as nat
@@ -474,6 +504,11 @@ def main_fhp(a, rank, world, local_rank):
     launches = nat.lib().prl_launch_count() - launches0
     n_allreduce = s.n_allreduce - n_ar0
     clocks = sampler.stop() if sampler else None
+    if a.dump_outputs and rank == 0:
+        s.flush_average()  # Vanilla / Linear CFR: the average a caller reads (state_dict) includes the pending part
+        dump_outputs(a.dump_outputs, {"exploitability": np.reshape(np.asarray(trace, np.float64), (-1, 3)),
+                                      "trunk_regret": s.bufs.regret, "trunk_strat": s.bufs.strat, "trunk_avg": s.bufs.avg},
+                     {"regret": s.regret, "avg": s.avg})
     t = torch.tensor([dev_ms], dtype=torch.float64, device="cuda")
     if world > 1:
         dist.barrier()
@@ -523,15 +558,9 @@ def main_fhp(a, rank, world, local_rank):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", HBM_PEAK_GBS))
     achieved = bytes_launch / (sweep_ms * 1e-3) / 1e9
-    traffic, traffic_note = None, "no ncu capture recorded under profiles/"
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "r02_fhp_sweep_traffic.json")))
-        traffic = tr["dram_bytes_per_board"] * s.n_boards
-        traffic_note = tr["note"]
-    except Exception:
-        pass
+    traffic, traffic_note = None, "DRAM traffic not measured"
     it_ms = max_ms / K
     # SURVEY.md §8(d): B_min = 16 R sum(A) + 4 R n_boards per iteration with R = 1326 (regret + average read and written once)
     b_min = (16 * 1326 * 14 + 4 * 1326) * (N_CLASSES if not a.fhp_boards else a.fhp_boards)
@@ -539,7 +568,7 @@ def main_fhp(a, rank, world, local_rank):
         "bound": "hbm", "kernel": "board_sweep_kernel<ShapeFHP, seat, update> (persistent, 2 CTAs per SM, one (board, seat) unit at a "
                                   "time; 2 launches per iteration = %.0f %% of the iteration)" % (100 * 2 * sweep_ms / (2 * half_ms)),
         "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-        "peak_source": "MEASURED_PEAKS.json" if "hbm_gbs" in peaks else "fallback 6.65 TB/s",
+        "peak_source": "MEASURED_PEAKS.json" if "hbm_gbs" in peaks else "H100 SXM data sheet 3.35 TB/s",
         "algorithmic_bytes_per_launch": bytes_launch, "launch_ms": sweep_ms, "traffic": traffic, "traffic_note": traffic_note,
         "bytes_per_board": {"rows": 35 * rows_bytes, "index_tables": L["blob"]},
         "frac_vs_Bmin": {"B_min_bytes_per_iteration": b_min * (1.0 / world if world > 1 else 1.0),
@@ -617,7 +646,7 @@ def main_fhp(a, rank, world, local_rank):
         "warmup": W, "ms_per_step": it_ms, "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32",
         "data": "synthetic (deterministic game tree, no dataset)",
         "config": dict(cfg, boards_per_rank=s_n_boards(nb_used, rank, world), engine="board-resident (pokerrl_b200/board_engine.py)",
-                       l2="per-rank tables %.1f GB >> 126 MB L2 (no explicit flush)" % (
+                       l2="per-rank tables %.1f GB >> 50 MB L2 (no explicit flush)" % (
                            2 * s_n_boards(nb_used, rank, world) * 14 * rows_bytes / 2 ** 30),
                        parallelism="boards round-robin over %d ranks; per bottom-up sweep ONE cross-rank sum of the chance node's "
                                    "int64 fixed-point vector (%d in the timed region): %s" % (world, n_allreduce, collective)),
@@ -678,12 +707,20 @@ def main():
     ap.add_argument("--algo", default="CFRPlus", choices=["CFRPlus", "LinearCFR", "VanillaCFR"],
                     help="fhp workload: the algorithm the board engine runs (the headline metric is CFRPlus)")
     ap.add_argument("--fhp-boards", type=int, default=0, help="debug: only the first n isomorphism classes")
-    ap.add_argument("--hulh-turns", type=int, default=0, help="hulh: only the first n turn cards (memory: the full 49 need >= 2 GPUs)")
+    ap.add_argument("--hulh-turns", type=int, default=0,
+                    help="hulh: only the first n turn cards (~5.3 GB each: at most 12 on one 80 GB GPU)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--converge", type=int, default=0, metavar="ITERS",
                     help="fhp / hulh: run ITERS iterations and print the exploitability-vs-wall-clock curve (one JSON line) "
                          "instead of the throughput line; evaluation every --eval-every iterations")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="fhp / hulh / Leduc throughput runs: after the timed steps write what they computed as "
+                         "DIR/<name>.npy (<= 64 MB, fixed seeded row sample; rank 0's boards when sharded)")
     a = ap.parse_args()
+    if a.steps is not None and a.steps < 1:
+        ap.error("--steps must be >= 1")
+    if a.dump_outputs and (a.workload in ("env", "handeval") or a.converge or a.impl == "reference"):
+        ap.error("--dump-outputs: throughput runs of fhp, hulh and the Leduc workloads on the GPU only")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -741,7 +778,8 @@ def main():
         }))
         return
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
+    import numpy as np
     import torch
     import torch.distributed as dist
     from pokerrl_b200 import _native as nat
@@ -835,6 +873,10 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     max_ms = float(t.item())
     n_allreduce = getattr(s, "n_allreduce", 0) - n_ar0
+    if a.dump_outputs and rank == 0:
+        b = s.bufs
+        dump_outputs(a.dump_outputs, {"exploitability": np.reshape(np.asarray(trace, np.float64), (-1, 3))},
+                     {"regret": b.regret, "strat": b.strat, "avg": b.avg})
 
     # --- roofline of the dominant kernels, timed live with CUDA events on their stream (sweep by sweep, after the run)
     import ctypes as C
@@ -845,8 +887,8 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    psrc = "MEASURED_PEAKS.json" if "hbm_gbs" in peaks else "fallback 6.65 TB/s"
+    peak = float(peaks.get("hbm_gbs", HBM_PEAK_GBS))
+    psrc = "MEASURED_PEAKS.json" if "hbm_gbs" in peaks else "H100 SXM data sheet 3.35 TB/s"
     if fhp:
         tree_p, buf_p = C.byref(s.dtree.desc), C.byref(s.bufs.desc)
         v_ms, r_ms = [], []
@@ -866,14 +908,10 @@ def main():
         vm, rm = statistics.mean(v_ms), statistics.mean(r_ms)
         achieved = vb / (vm * 1e-3) / 1e9
         roofline = {"bound": "hbm", "kernel": "value/regret sweep of one seat = fold2_kernel + terminal2_kernel_v3 + value2_kernel_v2<false,true> + "
-                    "chance_*_kernel over all %d levels (terminal2_kernel is the largest share, see profiles/)" % st["levels"],
+                    "chance_*_kernel over all %d levels" % st["levels"],
                     "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_source": psrc,
                     "algorithmic_bytes_per_sweep": vb, "sweep_ms": vm, "traffic": None,
-                    "traffic_note": "no full-game ncu --set full capture (110 GB resident; replay save/restore); the 20 000-"
-                    "board capture in profiles/r01_g_twocard_v2.md has terminal2_kernel at 25.1 KB DRAM per terminal row "
-                    "(10.6 KB of rows + the board's tables, shared by neighbouring rows through L2) and reach2_kernel_v2 "
-                    "at 22.9 KB per node on the widest level (3 rows in, 2 rows out = 26.5 KB algorithmic; part of a "
-                    "20 000-board level still sits in L2)",
+                    "traffic_note": "DRAM traffic not measured",
                     "reach_sweep": {"kernel": "reach2_kernel_v2<true> x %d levels" % st["levels"], "algorithmic_bytes": rb,
                                     "sweep_ms": rm, "achieved": rb / (rm * 1e-3) / 1e9, "frac": rb / (rm * 1e-3) / 1e9 / peak}}
     else:
@@ -957,7 +995,7 @@ def main():
         "scaling": "strong" if fhp else "weak", "vs_baseline": None, "dtype": "f32",
         "data": "synthetic (deterministic game tree, no dataset)",
         "config": dict(cfg, tree_per_rank=st,
-                       l2="per-rank working set %.1f GB >> 126 MB L2 (no explicit flush)" % (
+                       l2="per-rank working set %.1f GB >> 50 MB L2 (no explicit flush)" % (
                            (6 * st["nodes"] + 3 * st["sum_actions"]) * st["range"] * 4 / 2 ** 30),
                        parallelism=("boards sharded over %d ranks, one NCCL all-reduce of the chance-node sums per bottom-up "
                                     "sweep (%d in the timed region)" % (world, n_allreduce)) if fhp

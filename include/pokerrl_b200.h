@@ -1,5 +1,5 @@
 /*
- * pokerrl_b200 — C ABI of the B200-native tabular CFR / public-tree / best-response path.
+ * pokerrl_b200 — C ABI of the H100-native tabular CFR / public-tree / best-response path.
  *
  * Drop-in boundary (SURVEY.md §8b).  The reference has no native code on this path — its only FFI precedent is the
  * ctypes convention of PokerRL/_/CppWrapper.py:10-27 (caller allocates every buffer, native code only writes into
@@ -328,7 +328,7 @@ int prl_board_permute(const prl_board_game_t* g, int rows_per_board, const int64
  * missing board cards per terminal (ValueFiller.py:160-175 `_get_call_eq_preflop`, one-card games only); here the public
  * state's EQUITY MATRIX  E[h][h'] = sum over the sym_perm permutations q and the completions b of the board of
  * w_b * sign(rank_b(q(h)) - rank_b(q(h'))) (0 where a hand is blocked or the two hands share a card) is built once, stored
- * as three bf16 split planes in tcgen05 operand tiles, and every all-in terminal costs one column of a tensor-core GEMM
+ * as three bf16 split planes in wgmma operand tiles, and every all-in terminal costs one column of a tensor-core GEMM
  * (BASELINE.json north_star: "tensor cores used only for the dense 1326x1326 Hold'em showdown equity contraction").
  *   prl_allin_equity_accumulate: ec (DEVICE double[n_range][n_range], zeroed by the caller) += sum_b weight[b] * S_b for a chunk
  *     of boards; ranks DEVICE int32[n_boards][n_range] (prl_hand_rank_boards), weight DEVICE double[n_boards] (deal probability

@@ -1,6 +1,6 @@
 """Generate golden CFR / PublicTree fixtures by RUNNING THE REFERENCE ITSELF (TEST INFRASTRUCTURE).
 
-Run in the build container only (needs /root/reference):
+Run in the build container only (needs a PokerRL checkout in POKERRL_REFERENCE):
 
     python oracle/gen_golden_cfr.py            # writes tests/golden/*.npz
 

@@ -1,4 +1,4 @@
-"""Golden PokerEnv trajectories produced by RUNNING THE REFERENCE ENV (TEST INFRASTRUCTURE; needs /root/reference):
+"""Golden PokerEnv trajectories produced by RUNNING THE REFERENCE ENV (TEST INFRASTRUCTURE; needs a PokerRL checkout in POKERRL_REFERENCE):
 
     python oracle/gen_golden_env.py        # writes tests/golden/env_<game>.npz
 

@@ -1,5 +1,5 @@
 """Golden check-down equities for the LBR roll-out kernel, produced by RUNNING THE REFERENCE's _LBRRolloutManager
-(PokerRL/eval/lbr/LocalLBRWorker.py:377-512) on Hold'em states (TEST INFRASTRUCTURE; needs /root/reference):
+(PokerRL/eval/lbr/LocalLBRWorker.py:377-512) on Hold'em states (TEST INFRASTRUCTURE; needs a PokerRL checkout in POKERRL_REFERENCE):
 
     python oracle/gen_golden_lbr.py      # writes tests/golden/lbr_rollouts.npz
 

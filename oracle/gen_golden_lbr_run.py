@@ -1,5 +1,5 @@
 """Golden LBR EPISODES, produced by RUNNING THE REFERENCE's LocalLBRWorker (PokerRL/eval/lbr/LocalLBRWorker.py:12-308) against a
-deterministic hand-dependent policy (TEST INFRASTRUCTURE; needs /root/reference):
+deterministic hand-dependent policy (TEST INFRASTRUCTURE; needs a PokerRL checkout in POKERRL_REFERENCE):
 
     python oracle/gen_golden_lbr_run.py      # writes tests/golden/lbr_runs.npz
 

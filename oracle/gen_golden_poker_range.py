@@ -1,5 +1,5 @@
 """Golden traces of the REFERENCE's PokerRange (PokerRL/game/PokerRange.py:9-160) under a scripted sequence of the operations
-the LBR evaluator performs (TEST INFRASTRUCTURE; needs /root/reference):
+the LBR evaluator performs (TEST INFRASTRUCTURE; needs a PokerRL checkout in POKERRL_REFERENCE):
 
     python oracle/gen_golden_poker_range.py      # writes tests/golden/poker_range.npz
 

@@ -1,5 +1,5 @@
 """Golden terminal rows for TWO-HOLE-CARD games, anchored on the reference's own hand evaluator
-(TEST INFRASTRUCTURE; needs /root/reference):
+(TEST INFRASTRUCTURE; needs a PokerRL checkout in POKERRL_REFERENCE):
 
     python oracle/gen_golden_twocard.py      # writes tests/golden/twocard_rows.npz
 

@@ -1,7 +1,7 @@
 """Reference harness (TEST INFRASTRUCTURE ONLY — never imported by the product path).
 
-Imports the read-only PokerRL reference from /root/reference (only present in the build
-container, never on the GPU box) with the two stub packages under oracle/ref_stubs, and
+Imports a checkout of the PokerRL reference (directory given by POKERRL_REFERENCE; only the fixture generators need it,
+never the tests) with the two stub packages under oracle/ref_stubs, and
 provides helpers that flatten the reference's object tree (PokerRL/game/_/tree/nodes.py:8-62)
 into DFS-pre-order arrays so that golden fixtures can be committed under tests/golden/.
 
@@ -13,7 +13,7 @@ import sys
 
 import numpy as np
 
-REFERENCE_ROOT = os.environ.get("POKERRL_REFERENCE", "/root/reference")
+REFERENCE_ROOT = os.environ.get("POKERRL_REFERENCE", "")
 _STUBS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "ref_stubs")
 
 
@@ -24,7 +24,7 @@ def reference_available():
 def import_reference():
     """Put the reference and the gym/pycrayon stubs on sys.path. Returns the PokerRL module."""
     if not reference_available():
-        raise RuntimeError("PokerRL reference not found at %s" % REFERENCE_ROOT)
+        raise RuntimeError("PokerRL reference not found at %r: set POKERRL_REFERENCE to a PokerRL checkout" % REFERENCE_ROOT)
     for p in (_STUBS, REFERENCE_ROOT):
         if p not in sys.path:
             sys.path.insert(0, p)

@@ -1,5 +1,5 @@
 """Base of the full-width tabular CFR variants with the reference's constructor, schedule and log names
-(`PokerRL/cfr/_CFRBase.py:12-278`), driving the B200 engine (`pokerrl_b200.solver.CFRSolver`).
+(`PokerRL/cfr/_CFRBase.py:12-278`), driving the H100 engine (`pokerrl_b200.solver.CFRSolver`).
 
 Differences to the reference, none of which changes a logged number:
   * one flat HBM-resident tree per stack size instead of Python node objects; the per-iteration rebuild of a fresh

@@ -1,4 +1,4 @@
-// All-in showdowns before the board is complete, two-hole-card games - sm_100a (tcgen05 tensor cores, TMEM, TMA bulk copies).
+// All-in showdowns before the board is complete, two-hole-card games - sm_90a (wgmma tensor cores, TMA bulk copies, mbarrier).
 //
 // Reference: ValueFiller.py:160-175 (`_get_call_eq_preflop`, one-card games: the missing board card is enumerated per
 // terminal and the per-board showdown rows of ValueFiller.py:127-158 are averaged).  For two-card hands the enumeration is
@@ -9,17 +9,17 @@
 // place of this path where tensor cores are the right tool (BASELINE.json north_star).
 //
 // Precision: fp32 operands are split into three bf16 planes (8 + 8 + 8 mantissa bits); the six products of total order
-// <= 2 (hi*hi, hi*mid, mid*hi, hi*lo, mid*mid, lo*hi) accumulate in fp32 in tensor memory: ~2^-22 of the row's mass, the
+// <= 2 (hi*hi, hi*mid, mid*hi, hi*lo, mid*mid, lo*hi) accumulate in fp32 registers: ~2^-22 of the row's mass, the
 // level of an fp32 dot product (test: tests/test_gpu_allin.py against float64).
 //
 // Kernels:
 //   allin_accum_kernel   Ec += sum_b w_b S_b over a chunk of boards, 64 x 64 tile per CTA, double accumulators
-//   allin_tiles_kernel   symmetrise over q, mask card-sharing pairs, 3-way bf16 split, write tcgen05 operand tiles
+//   allin_tiles_kernel   symmetrise over q, mask card-sharing pairs, 3-way bf16 split, write wgmma operand tiles
 //                        (K-major, no swizzle: 8 x 16-byte core matrices; a 128 x 64 tile is 16 KB contiguous, fetched by
 //                        ONE cp.async.bulk)
 //   allin_gemm_kernel    CTA (m-tile of 128 hands, k-block of 64 hands): A tiles by TMA bulk copy on an mbarrier, B (the
-//                        <= 16 reach rows, split on the fly) built in shared memory, 24 tcgen05.mma (M128 N16 K16, bf16 ->
-//                        fp32 in TMEM) issued by one thread, tcgen05.commit -> mbarrier, tcgen05.ld epilogue -> partial sums
+//                        <= 16 reach rows, split on the fly) built in shared memory; two warpgroups, each 24 wgmma
+//                        (M64 N16 K16, bf16 -> fp32 registers) over its 64 rows of the m-tile -> partial sums
 //   allin_finish_kernel  fixed-order sum of the 21 k-block partials, scale, write the ev / ev_br rows
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -30,13 +30,13 @@
 
 namespace {
 
-constexpr int kTileM = 128, kTileK = 64, kCols = 16;       // UMMA M, k-block, UMMA N (reach rows per launch)
+constexpr int kTileM = 128, kTileK = 64, kCols = 16;       // m-tile, k-block, wgmma N (reach rows per launch)
 constexpr int kSplits = 3;
 constexpr int kATileBytes = kTileM * kTileK * 2;           // 16 KB per split plane
 constexpr int kBTileBytes = kCols * kTileK * 2;            // 2 KB per split plane
 constexpr int kLBO = 128, kSBO = (kTileK / 8) * 128;       // core matrices: adjacent in K / adjacent 8-row groups (bytes)
-constexpr int kGemmThreads = 128;
-constexpr int kTmemCols = 32;                              // power of two >= 32; 16 used
+constexpr int kWgM = 64;                                   // wgmma M: rows of the m-tile per warpgroup
+constexpr int kGemmThreads = 128 * (kTileM / kWgM);        // two warpgroups
 
 inline int m_tiles(int R) { return (R + kTileM - 1) / kTileM; }
 inline int k_blocks(int R) { return (R + kTileK - 1) / kTileK; }
@@ -69,42 +69,24 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot, uint32_t cols) {  // one whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {  // the same warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; one thread issues for the CTA
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// d (+)= A[smem] * B[smem], both K-major bf16, fp32 accumulators in registers; issued by the whole warpgroup
+__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t a_desc, uint64_t b_desc) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a_desc), "l"(b_desc), "r"(1)
         : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {  // arrives on the mbarrier when all MMAs issued so far are done
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {  // lane = TMEM lane of this warp's quarter
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
-// shared-memory matrix descriptor, K-major, no swizzle (cute::UMMA::SmemDescriptor, version 1): start address, leading
-// (K-adjacent core matrices) and stride (8-row groups) byte offsets, all >> 4
+// wgmma shared-memory matrix descriptor, K-major, no swizzle (layout type 0): start address, leading (K-adjacent core
+// matrices) and stride (8-row groups) byte offsets, all >> 4
 __device__ __forceinline__ uint64_t smem_desc(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(kLBO >> 4) << 16) | ((uint64_t)(kSBO >> 4) << 32) | (1ull << 46);
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(kLBO >> 4) << 16) | ((uint64_t)(kSBO >> 4) << 32);
 }
-// instruction descriptor (cute::UMMA::InstrDescriptor): D fp32, A / B bf16, both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-constexpr uint32_t kIdesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(kCols >> 3) << 17) | ((uint32_t)(kTileM >> 4) << 24);
 
 // element (row r of the tile, column k of the k-block) inside a K-major no-swizzle operand tile, in bf16 elements
 __host__ __device__ __forceinline__ int tile_elem(int r, int k) { return (r >> 3) * (kSBO / 2) + (k >> 3) * (kLBO / 2) + (r & 7) * 8 + (k & 7); }
@@ -214,32 +196,21 @@ __global__ void __launch_bounds__(kGemmThreads) allin_gemm_kernel(const GemmArgs
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned char* sA = smem;                                  // 3 planes x 16 KB
     unsigned char* sB = smem + kSplits * kATileBytes;          // 3 planes x 2 KB
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sB + kSplits * kBTileBytes);  // [0]: A landed, [1]: MMAs done
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    uint64_t* bar = reinterpret_cast<uint64_t*>(sB + kSplits * kBTileBytes);  // A landed
+    const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
     const int mt = blockIdx.x, kb = blockIdx.y;
 
     if (tid == 0) {
-        mbar_init(&bars[0], 1);
-        mbar_init(&bars[1], 1);
+        mbar_init(bar, 1);
         fence_barrier_init();
-        fence_async_shared();
     }
-    if (warp == 0) {
-        __syncwarp();
-        tmem_alloc(tmem_slot, kTmemCols);
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-
     if (tid == 0) {  // the three planes of this (m-tile, k-block) are contiguous: one 48 KB bulk copy
-        mbar_expect_tx(&bars[0], kSplits * kATileBytes);
-        bulk_g2s(sA, a.tiles + (size_t)(mt * a.KB + kb) * kSplits * (kTileM * kTileK), kSplits * kATileBytes, &bars[0]);
+        mbar_expect_tx(bar, kSplits * kATileBytes);
+        bulk_g2s(sA, a.tiles + (size_t)(mt * a.KB + kb) * kSplits * (kTileM * kTileK), kSplits * kATileBytes, bar);
     }
-    // B: thread (n = tid / 8, 8 consecutive k) - one 16-byte core-matrix row per plane
-    {
+    // B: thread (n = tid / 8, 8 consecutive k) of the first warpgroup - one 16-byte core-matrix row per plane
+    if (tid < kCols * (kTileK / 8)) {
         const int n = tid >> 3, k0 = (tid & 7) * 8;
         const float* xr = a.x[n];
         __align__(16) __nv_bfloat16 p[kSplits][8];
@@ -255,39 +226,31 @@ __global__ void __launch_bounds__(kGemmThreads) allin_gemm_kernel(const GemmArgs
     }
     fence_async_shared();  // generic-proxy writes of B -> visible to the tensor core (async proxy)
     __syncthreads();
+    mbar_wait(bar, 0);
 
-    if (tid == 0) {
-        mbar_wait(&bars[0], 0);
-        tc_fence_after();
-        const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
-        // (plane of E, plane of x): the six products of total order <= 2, largest last is not required - fp32 accumulation
-        const int pa[6] = {2, 0, 1, 1, 0, 0}, pb[6] = {0, 2, 1, 0, 1, 0};
-        uint32_t acc = 0;
+    // warpgroup wg: rows 64 wg .. 64 wg + 63 of the m-tile = 8 core-matrix row groups further into each A plane
+    float d[8];
 #pragma unroll
-        for (int t = 0; t < 6; ++t)
+    for (int i = 0; i < 8; ++i) d[i] = 0.0f;
+    const uint32_t a0 = smem_u32(sA) + wg * (kWgM / 8) * kSBO, b0 = smem_u32(sB);
+    // (plane of E, plane of x): the six products of total order <= 2, largest last is not required - fp32 accumulation
+    const int pa[6] = {2, 0, 1, 1, 0, 0}, pb[6] = {0, 2, 1, 0, 1, 0};
+    wgmma_fence();
 #pragma unroll
-            for (int ks = 0; ks < kTileK / 16; ++ks) {  // K = 16 per instruction: two core matrices = 256 bytes along K
-                const uint64_t da = smem_desc(a0 + pa[t] * kATileBytes + ks * 2 * kLBO);
-                const uint64_t db = smem_desc(b0 + pb[t] * kBTileBytes + ks * 2 * kLBO);
-                umma_bf16(tmem, da, db, kIdesc, acc);
-                acc = 1;
-            }
-        umma_commit(&bars[1]);
+    for (int t = 0; t < 6; ++t)
+#pragma unroll
+        for (int ks = 0; ks < kTileK / 16; ++ks)  // K = 16 per instruction: two core matrices = 256 bytes along K
+            wgmma_m64n16k16(d, smem_desc(a0 + pa[t] * kATileBytes + ks * 2 * kLBO), smem_desc(b0 + pb[t] * kBTileBytes + ks * 2 * kLBO));
+    wgmma_commit();
+    wgmma_wait_all();
+    // epilogue: accumulator i of lane l in warp w holds row 16 w + l / 4 + 8 (i / 2 % 2), column 8 (i / 4) + 2 (l % 4) + i % 2
+    float* out = a.partial + (size_t)kb * kCols * (a.MT * kTileM);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const int m = mt * kTileM + wg * kWgM + warp * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+        const int n = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        out[(size_t)n * (a.MT * kTileM) + m] = d[i];
     }
-    mbar_wait(&bars[1], 0);
-    __syncwarp();  // tcgen05.ld is .sync.aligned: the issuing thread rejoins its warp first
-    tc_fence_after();
-    {   // epilogue: warp w owns TMEM lanes 32 w .. 32 w + 31 = rows of the m-tile; 16 columns = the reach rows
-        uint32_t r[16];
-        tmem_ld16(tmem + ((uint32_t)(warp * 32) << 16), r);
-        const int m = mt * kTileM + warp * 32 + lane;
-        float* out = a.partial + (size_t)kb * kCols * (a.MT * kTileM) + m;
-#pragma unroll
-        for (int n = 0; n < kCols; ++n) out[(size_t)n * (a.MT * kTileM)] = __uint_as_float(r[n]);
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, kTmemCols);
 }
 
 struct FinishArgs {

@@ -1,8 +1,8 @@
-"""Builds pokerrl_b200/lib/libpokerrl_b200.so with nvcc for sm_100a (in-tree, no JIT cache).
+"""Builds pokerrl_b200/lib/libpokerrl_b200.so with nvcc for sm_90a (H100; in-tree, no JIT cache).
 
     python -m pokerrl_b200.csrc.build            # or: python pokerrl_b200/csrc/build.py [--force]
 
-nvcc cross-compiles without a GPU.  The .so is git-ignored but travels to the GPU box with the snapshot.
+nvcc cross-compiles without a GPU.  The .so and the objects under pokerrl_b200/lib/ are build products (git-ignored).
 """
 import os
 import subprocess
@@ -13,7 +13,7 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 LIB_DIR = os.path.join(os.path.dirname(HERE), "lib")
 LIB = os.path.join(LIB_DIR, "libpokerrl_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include"), "-I", HERE]
 
 # translation unit -> extra flags.  The CFR sweeps must not contract multiply-adds (bit parity with numpy).
@@ -47,7 +47,7 @@ def build(force=False, verbose=False):
         s = os.path.join(HERE, src)
         o = os.path.join(obj_dir, src.replace(".cu", ".o").replace(".cpp", ".o"))
         objs.append(o)
-        if force or _stale(o, [s] + headers):
+        if force or _stale(o, [s, os.path.abspath(__file__)] + headers):  # a change of ARCH / flags rebuilds
             cmd = [NVCC] + ARCH + COMMON + extra + (["-Xptxas", "-v"] if verbose else []) + ["-c", s, "-o", o]
             print(" ".join(cmd))
             subprocess.check_call(cmd)

@@ -1,7 +1,7 @@
-// Board-resident CFR+ sweeps for two-hole-card games with ONE chance layer (Flop5Holdem, PokerRL/game/games.py:222-254) - sm_100a.
+// Board-resident CFR+ sweeps for two-hole-card games with ONE chance layer (Flop5Holdem, PokerRL/game/games.py:222-254) - sm_90a.
 //
 // The level-synchronous sweeps (cfr_twocard.cu) spill every node vector of every board subtree to HBM: 186 GB per
-// iteration against 40 GB of regret / average tables (VERDICT r01).  Here ONE persistent CTA walks whole (board, seat)
+// iteration against 40 GB of regret / average tables.  Here ONE persistent CTA walks whole (board, seat)
 // units: the 15-node post-deal subtree of a board lives in registers / shared memory, HBM sees only
 //     opponent regret rows (strategy by regret matching)  ->  reach of the opponent, top-down        (P1)
 //     9 terminal rows (5 showdown + 4 fold) evaluated together in shared memory                      (P2)
@@ -48,7 +48,7 @@ constexpr int kBlobA = kRecBytes + kShBytes;                // 10 880 B, needed 
 constexpr int kBlobBytes = kBlobA + kRowIdxBytes;           // 15 392 B
 static_assert(kBlobA % 16 == 0 && kRowIdxBytes % 16 == 0, "bulk copies move multiples of 16 bytes");
 
-// kernel variants (A/B switches; the defaults are the measured winners, profiles/r02_q_sweep_variants.md)
+// kernel variants (A/B switches, tools/build_variants.py; the defaults are the variants kept)
 #ifndef PRL_BV_RED
 #define PRL_BV_RED 1         // chance sums by 64-bit RED instead of load + add + store
 #endif
@@ -70,7 +70,7 @@ static_assert(kBlobA % 16 == 0 && kRowIdxBytes % 16 == 0, "bulk copies move mult
 #endif
 constexpr int kVP1Pipe = PRL_BV_P1PIPE;
 constexpr bool kVRed = PRL_BV_RED, kVFoldLin = PRL_BV_FOLDLIN, kVErT = PRL_BV_ERT;
-// measured and removed (profiles/r02_q_sweep_variants.md): five-warp / one-warp-per-vector scans, the single-warp stage spread
+// tried and removed: five-warp / one-warp-per-vector scans, the single-warp stage spread
 // over nine warps, the third P3 pass spread over all warps, two positions requested a unit ahead
 
 constexpr int kThreads = 384;  // 12 warps; 3 strength positions per thread (3 * 384 = 1152 >= 1081: 94 % of the lanes busy)
@@ -79,12 +79,27 @@ constexpr int kWarps = kThreads / 32;
 
 // ---- compiled shape of the post-deal subtree (breadth-first; Flop5Holdem with pot-size raises, stacks that allow the
 //      full raise sequence).  The host checks the game's abstract tree against these arrays.
+// per-node tables packed 4 bits per node (value + 1): a lookup is a shift, never a local-memory array
+struct Nodes15 {
+    int v[15];
+};
+constexpr unsigned long long pack_nodes(Nodes15 t) {
+    unsigned long long r = 0;
+    for (int i = 0; i < 15; ++i) r |= (unsigned long long)(t.v[i] + 1) << (4 * i);
+    return r;
+}
+constexpr int unpack_node(unsigned long long t, int i) { return (int)((t >> (4 * i)) & 0xF) - 1; }
+
 struct ShapeFHP {
     static constexpr int N = 15;
-    static constexpr int kind(int i) { constexpr int a[N] = {1, 0, 0, 4, 1, 3, 4, 1, 3, 4, 0, 3, 4, 3, 4}; return a[i]; }
-    static constexpr int parent(int i) { constexpr int a[N] = {-1, 0, 0, 1, 1, 2, 2, 2, 4, 4, 4, 7, 7, 10, 10}; return a[i]; }
-    static constexpr int first_child(int i) { constexpr int a[N] = {1, 3, 5, -1, 8, -1, -1, 11, -1, -1, 13, -1, -1, -1, -1}; return a[i]; }
-    static constexpr int n_children(int i) { constexpr int a[N] = {2, 2, 3, 0, 3, 0, 0, 2, 0, 0, 2, 0, 0, 0, 0}; return a[i]; }
+    static constexpr unsigned long long kKind = pack_nodes({{1, 0, 0, 4, 1, 3, 4, 1, 3, 4, 0, 3, 4, 3, 4}});
+    static constexpr unsigned long long kParent = pack_nodes({{-1, 0, 0, 1, 1, 2, 2, 2, 4, 4, 4, 7, 7, 10, 10}});
+    static constexpr unsigned long long kFirstChild = pack_nodes({{1, 3, 5, -1, 8, -1, -1, 11, -1, -1, 13, -1, -1, -1, -1}});
+    static constexpr unsigned long long kNChildren = pack_nodes({{2, 2, 3, 0, 3, 0, 0, 2, 0, 0, 2, 0, 0, 0, 0}});
+    static constexpr int kind(int i) { return unpack_node(kKind, i); }
+    static constexpr int parent(int i) { return unpack_node(kParent, i); }
+    static constexpr int first_child(int i) { return unpack_node(kFirstChild, i); }
+    static constexpr int n_children(int i) { return unpack_node(kNChildren, i); }
     // index of terminal i among the showdown / fold vectors
     static constexpr int vec_index(int i) {
         int n = 0;
@@ -156,7 +171,7 @@ constexpr int kRowTotBytes = ShapeFHP::n_sd * kRowPad * 8;
 constexpr int kBarOff = kRowTotOff + kRowTotBytes;                          // 3 mbarriers
 constexpr int kSmemBytes = kBarOff + 32;
 static_assert(kBlobOff % 16 == 0 && kRowIdxOff % 16 == 0 && kCsdOff % 8 == 0 && kMiscOff % 8 == 0 && kRowTotOff % 8 == 0 && kBarOff % 8 == 0, "alignment");
-static_assert(2 * (kSmemBytes + 1024) <= 233472, "two CTAs per SM");
+static_assert(2 * (kSmemBytes + 1024) <= 233472, "two CTAs per SM (228 KB of shared memory per H100 SM)");
 
 struct SweepArgs {
     prl_board_game_t g;
@@ -354,9 +369,10 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
                     if constexpr (SH::kind(n) <= 1) {
                         constexpr int fc = SH::first_child(n);
                         if constexpr (SH::kind(n) == OPP) {
+                            constexpr int r0 = SH::row_of(fc);  // the node's children own rows r0 .. r0 + A - 1
                             float gg[A], s[A];
 #pragma unroll
-                            for (int c = 0; c < A; ++c) gg[c] = gk[SH::row_of(fc + c) - OPP0];
+                            for (int c = 0; c < A; ++c) gg[c] = gk[r0 - OPP0 + c];
                             node_strategy<A>(gg, asis_opp, s);
 #pragma unroll
                             for (int c = 0; c < A; ++c) x[fc + c] = x[n] * s[c];
@@ -365,7 +381,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
                                     float* arow = G.avg + (size_t)j * kBoardFloats + i;
 #pragma unroll
                                     for (int c = 0; c < A; ++c) {
-                                        float* ap = arow + (size_t)SH::row_of(fc + c) * kLdb;
+                                        float* ap = arow + (size_t)(r0 + c) * kLdb;
                                         st_stream(ap, __fadd_rn(ld_stream(ap), __fmul_rn(x[fc + c], a.defer_w)));
                                     }
                                 }
@@ -1001,7 +1017,7 @@ int default_grid() {
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) dev = 0;
     if (!cached[dev]) {
-        int sms = 148;
+        int sms = 132;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         cached[dev] = 2 * sms;
     }

@@ -1,4 +1,4 @@
-// Level-synchronous public-tree sweeps for tabular CFR / best response, one-hole-card games (sm_100a).
+// Level-synchronous public-tree sweeps for tabular CFR / best response, one-hole-card games (sm_90a).
 //
 // Mapping: ONE LANE PER (NODE, HAND); a warp holds 32 / R whole nodes (5 for Leduc's R = 6, 1 for BigLeduc's R = 24),
 // taken from a per-level work list sorted by node kind (no divergence).  Nodes of one depth are contiguous, children of
@@ -476,7 +476,7 @@ __device__ __forceinline__ void root_exploitability(const prl_tree_t& T, const p
 }
 
 // THREADS: block size = threads per SM (one block per SM): 512 at 128 registers per thread.  A 1024-thread / 64-register
-// instantiation measured 1 668 vs 1 677 iterations/s on the B_5 tree (profiles/r02_h_leduc_schedules.md) and was removed.
+// instantiation was no faster on the B_5 tree and was removed.
 template <int R, int NS, int THREADS>
 __global__ void __launch_bounds__(THREADS, 1) cfr_iterations_kernel(Ctx c, const Levels lv, const int n_iters) {
     cg::grid_group grid = cg::this_grid();

@@ -1,4 +1,4 @@
-// Level-synchronous public-tree sweeps for TWO-HOLE-CARD games (Hold'em family, range R = C(deck,2) = 1326) - sm_100a.
+// Level-synchronous public-tree sweeps for TWO-HOLE-CARD games (Hold'em family, range R = C(deck,2) = 1326) - sm_90a.
 //
 // The reference has no working value path for these games (ValueFiller.py:18-19 and PublicTree.py:193-203 are
 // one-card only); the arithmetic here is the generalisation stated in SURVEY.md appendix A and restated in float64 by
@@ -715,8 +715,7 @@ __global__ void __launch_bounds__(kTermThreads) terminal2_kernel(const Ctx2 c) {
 // v3: the v2 arithmetic with every input of a showdown row STAGED IN SHARED MEMORY BY ASYNCHRONOUS COPIES (cp.async):
 // the opponent's reach row and the board's three tables (strength positions, card-row orders, packed hand records) are
 // requested together right after ONE structure load (work_rec2), so a terminal row pays two dependent global latencies
-// (record -> everything) instead of five (order -> node fields -> reach row -> row orders -> hand records); the ncu
-// capture of v2 had 56 % of its stall samples on exactly those loads (profiles/r01_g_twocard_v2.md).
+// (record -> everything) instead of five (order -> node fields -> reach row -> row orders -> hand records).
 __device__ __forceinline__ void cp_async4(void* dst, const void* src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
 }

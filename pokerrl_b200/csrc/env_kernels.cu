@@ -1,4 +1,4 @@
-// Batched heads-up PokerEnv: reset / step for B independent tables, one thread per table (sm_100a).
+// Batched heads-up PokerEnv: reset / step for B independent tables, one thread per table (sm_90a).
 //
 // Restates the reference's scalar Python engine for two seats (SURVEY.md appendix B), integer chip accounting:
 //   reset            PokerRL/game/_/rl_env/base/PokerEnv.py:1075-1122        legalisation  PokerEnv.py:885-941

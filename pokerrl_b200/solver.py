@@ -19,7 +19,7 @@ def _require_cuda(device):
     """torch.device of the GPU to use: the given one, else the process's CURRENT device (under torchrun each rank sets
     its own with torch.cuda.set_device; never silently cuda:0)."""
     if not torch.cuda.is_available():
-        raise RuntimeError("pokerrl_b200 needs a CUDA device (sm_100a); there is no CPU fallback.")
+        raise RuntimeError("pokerrl_b200 needs a CUDA device (sm_90a); there is no CPU fallback.")
     d = torch.device(device if device is not None else "cuda:%d" % torch.cuda.current_device())
     if d.type != "cuda":
         raise RuntimeError("pokerrl_b200 runs on CUDA devices only, got %r" % (device,))
@@ -73,7 +73,7 @@ class DeviceTree:
         self.device = _require_cuda(device)
         rules = ft.rules
         self.R = ft.R
-        # row stride: R for the one-card games (measured on B200: padding Leduc rows 6 -> 8 floats was 8 % slower);
+        # row stride: R for the one-card games (padding Leduc rows 6 -> 8 floats only adds bytes to a latency-bound sweep);
         # two-card rows (R = 1326) are padded to a multiple of 4 floats so that every row starts 16-byte aligned
         self.ld = ft.R if rules.N_HOLE_CARDS == 1 else -(-ft.R // 4) * 4
         dev = self.device

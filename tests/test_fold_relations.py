@@ -11,14 +11,14 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 
 def _c_array(src, name):
-    m = re.search(r"%s\(int i\) \{ constexpr int a\[N\] = \{([^}]*)\}" % name, src)
+    m = re.search(r"%s = pack_nodes\(\{\{([^}]*)\}\}\)" % name, src)
     return [int(x) for x in m.group(1).split(",")]
 
 
 def test_fold_relation_table_of_the_kernel_is_the_derived_one():
     import fold_relations as fr
     src = open(os.path.join(ROOT, "pokerrl_b200", "csrc", "cfr_board.cu")).read()
-    assert _c_array(src, "kind") == fr.KIND and _c_array(src, "first_child") == fr.FIRST and _c_array(src, "n_children") == fr.NCH
+    assert _c_array(src, "kKind") == fr.KIND and _c_array(src, "kFirstChild") == fr.FIRST and _c_array(src, "kNChildren") == fr.NCH
     m = re.search(r"constexpr int c\[2\]\[4\]\[5\] = (\{\{.*?\}\}\});", src, re.S)
     got = np.array(eval(m.group(1).replace("{", "[").replace("}", "]").rstrip(";")))
     want = fr.derive()

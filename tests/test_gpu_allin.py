@@ -1,4 +1,4 @@
-"""GPU parity of the all-in showdown before the deal (csrc/allin_dense.cu: equity matrix, tcgen05 GEMM) through the C ABI.
+"""GPU parity of the all-in showdown before the deal (csrc/allin_dense.cu: equity matrix, wgmma GEMM) through the C ABI.
 
 Oracle: float64 brute force (oracle/cfr2_numpy.allin_equity_matrix) on hand strengths of the REFERENCE's lib_hand_eval.so
 (tests/golden/twocard_rows.npz `ranks`) - the one-card analogue in the reference is ValueFiller.py:160-175.

@@ -1,8 +1,7 @@
 """GPU parity of the two-card (Hold'em family) LEVEL-engine sweeps against the float64 oracle (oracle/cfr2_numpy.py, whose
 terminal rows are pinned on the reference's hand strengths, tests/test_oracle_twocard_rows.py).
 
-Tolerances (achieved errors are printed with -s; measured on B200: reach 2e-8, values 1.6e-7, regrets over four free-running
-iterations <= 5.4e-7, exploitability <= 2.2e-7 incl. the multi-street sub-game): BASELINE.json's bar, 1e-6 of the largest
+Tolerances (achieved errors are printed with -s): BASELINE.json's bar, 1e-6 of the largest
 magnitude of the compared array / relative for exploitability; regrets of free-running iterations 2 and 3 and the trunk
 regrets of the isomorphism test get 2e-6 / 5e-6 (float32 round-off decides ties in regret matching, SURVEY headline 5)."""
 import numpy as np

@@ -10,7 +10,7 @@ sys.path.insert(0, ROOT)
 from pokerrl_b200.csrc import build as B  # noqa: E402
 
 # switches left in csrc/cfr_board.cu: each accepted change against its predecessor (the rejected ones were removed from the
-# source; profiles/r02_q_sweep_variants.md keeps their numbers)
+# source)
 _ON = dict(RED=1, P1PIPE=1, FOLDLIN=1, ERT=1, ROWTOTF=1, NEWTON=1)
 VARIANTS = {
     "final": dict(_ON),
