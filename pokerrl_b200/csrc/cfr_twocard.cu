@@ -13,6 +13,9 @@
 //             strictly-stronger mass from group boundaries, minus a ~100-term blocker correction per hand
 // instead of the O(R^2) sign-matrix product: these rows are HBM-bound, the dense 1326x1326 contraction (tensor cores)
 // would only add work - see DESIGN.md §6.
+// Each operation (reach, decision nodes with the CFR rules, showdown steps) is written once as a device body; the
+// record-based kernels (*_v2, terminal2_kernel_v3) and the record-free ones differ only in how they read a node's
+// structure (16-byte records or pointer chains) and the board's tables (packed hand records or separate tables).
 #include <cuda_runtime.h>
 #include <vector>
 #include <stdint.h>
@@ -84,172 +87,56 @@ __device__ __forceinline__ bool hand_blocked(const prl_tree_t& T, int h, unsigne
     return ((bmask >> c1) | (bmask >> c2)) & 1ull;
 }
 
+// ------------------------------------------------------------------------------------------------ CFR rules
+// new regret of one (row, hand) from the instantaneous regret d = v(child) - v(node) and the stored regret; w = iter + 1
+__device__ __forceinline__ float regret_step(int algo, float d, float old, float w) {
+    if (algo == PRL_ALGO_CFR_PLUS) return fmaxf(d + old, 0.0f);
+    if (algo == PRL_ALGO_LINEAR) return w * d + old;
+    return d + old;
+}
+
+// regret matching of one node's rows: a row's positive regret over the node's positive regret mass, uniform where that
+// mass is 0
+struct RegretMatch {
+    F4 ssum, inv;
+    float uni;
+    __device__ __forceinline__ RegretMatch(const F4& pos_mass, int A) : ssum(pos_mass), uni(1.0f / (float)A) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) inv.v[i] = (ssum.v[i] > 0.0f) ? 1.0f / ssum.v[i] : 0.0f;
+    }
+    __device__ __forceinline__ F4 operator()(const F4& r) const {
+        F4 st;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) st.v[i] = (ssum.v[i] > 0.0f) ? fmaxf(r.v[i], 0.0f) * inv.v[i] : uni;
+        return st;
+    }
+};
+
+// average-strategy update of table row ap from the row's strategy s and the child's reach r
+__device__ __forceinline__ void avg_update(const Ctx2& c, float* ap, const F4& s, const F4& r) {
+    if (c.algo == PRL_ALGO_CFR_PLUS) {  // CFRPlus.py:65-87 (float table)
+        if (c.iter >= c.delay) {
+            F4 a = ld4(ap);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) a.v[i] = c.m_old * a.v[i] + c.m_new * s.v[i];
+            st4(ap, a);
+        }
+    } else {
+        F4 a = ld4(ap);
+        const float w = (c.algo == PRL_ALGO_LINEAR) ? (float)(c.iter + 1) : 1.0f;  // LinearCFR.py:56-61
+#pragma unroll
+        for (int i = 0; i < 4; ++i) a.v[i] = a.v[i] + r.v[i] * w;  // VanillaCFR.py:57-62
+        st4(ap, a);
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ reach (top-down)
-// block x = child node n of the level, thread = four hands; StrategyFiller.py:118-146 generalised
+// reach rows of node n for hands h0..h0+3 (StrategyFiller.py:118-146 generalised).  Structure of n: parent par, n's table
+// row `slot`, first table row fs of its siblings, kind pk and fan-out A of the parent (read only when par >= 0).
 template <bool UPDATE_AVG>
-__global__ void __launch_bounds__(kVecThreads) reach2_kernel(const Ctx2 c) {
+__device__ __forceinline__ void reach_rows(const Ctx2& c, int n, int h0, int par, int slot, int fs, int pk, int A) {
     const int ld = c.T.ld, R = c.T.n_range;
-    const int n = c.lo + blockIdx.x;
-    const int h0 = 4 * (blockIdx.y * blockDim.x + threadIdx.x);
-    if (h0 >= R) return;
     const size_t N = (size_t)c.T.n_nodes;
-    const int par = c.T.parent[n];
-#pragma unroll 1
-    for (int q = 0; q < 2; ++q) {
-        if (!(c.mask & (1 << q))) continue;
-        float* reach_q = c.B.reach + (size_t)q * N * ld;
-        F4 r;
-        if (par < 0) {  // PublicTree.py:122-124; a sub-game root that already shows a board zeroes the blocked hands
-            const int b = c.T.board[n];
-            const unsigned long long bm = (b >= 0) ? c.T.board_mask[b] : 0ull;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) r.v[i] = (h0 + i < R && !hand_blocked(c.T, h0 + i, bm)) ? 1.0f / (float)R : 0.0f;
-        } else {
-            const F4 rp = ld4(reach_q + (size_t)par * ld + h0);
-            const int pk = c.T.kind[par];
-            if (pk == PRL_KIND_CHANCE) {  // the deal multiplies both rows and zeroes hands holding a board card
-                const int b = c.T.board[n];
-                const unsigned long long bm = c.T.board_mask[b];
-                const float pr = c.T.board_prob[b];
-#pragma unroll
-                for (int i = 0; i < 4; ++i) r.v[i] = (h0 + i < R && !hand_blocked(c.T, h0 + i, bm)) ? rp.v[i] * pr : 0.0f;
-            } else if (pk == q) {
-                const int slot = c.T.slot[n];
-                const int m = c.mode[q];
-                const int fs = c.T.slot[c.T.first_child[par]];
-                const F4 s = strat4(c, m, slot, fs, c.T.n_children[par], h0);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) r.v[i] = s.v[i] * rp.v[i];
-                if (UPDATE_AVG && q == c.upd_p) {
-                    float* ap = (float*)c.B.avg + (size_t)slot * ld + h0;
-                    if (c.algo == PRL_ALGO_CFR_PLUS) {  // CFRPlus.py:65-87 (float table)
-                        if (c.iter >= c.delay) {
-                            F4 a = ld4(ap);
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) a.v[i] = c.m_old * a.v[i] + c.m_new * s.v[i];
-                            st4(ap, a);
-                        }
-                    } else {
-                        F4 a = ld4(ap);
-                        const float w = (c.algo == PRL_ALGO_LINEAR) ? (float)(c.iter + 1) : 1.0f;  // LinearCFR.py:56-61
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) a.v[i] = a.v[i] + r.v[i] * w;  // VanillaCFR.py:57-62
-                        st4(ap, a);
-                    }
-                }
-            } else {
-                r = rp;
-            }
-        }
-        st4(reach_q + (size_t)n * ld + h0, r);
-    }
-}
-
-// ------------------------------------------------------------------------------------------------ decision nodes (bottom-up)
-// block x = work-list entry t -> decision node n, thread = four hands; ValueFiller.py:80-93 + _CFRBase.py:146-185 +
-// regret matching
-template <bool WITH_BR, bool UPDATE>
-__global__ void __launch_bounds__(kVecThreads) value2_kernel(const Ctx2 c) {
-    const int ld = c.T.ld;
-    const int h0 = 4 * (blockIdx.y * blockDim.x + threadIdx.x);
-    if (h0 >= c.T.n_range) return;
-    const int n = c.T.order[c.lo + blockIdx.x];
-    const size_t N = (size_t)c.T.n_nodes;
-    const int kind = c.T.kind[n], fc = c.T.first_child[n], A = c.T.n_children[n];
-    const int fs = c.T.slot[fc];
-#pragma unroll 1
-    for (int p = 0; p < 2; ++p) {
-        if (!(c.mask & (1 << p))) continue;
-        float* ev_p = c.B.ev + (size_t)p * N * ld;
-        float* evbr_p = WITH_BR ? c.B.ev_br + (size_t)p * N * ld : nullptr;
-        const float* ecol = ev_p + (size_t)fc * ld + h0;
-        F4 v = splat(0.0f), vbr = splat(0.0f);
-        if (kind != p) {  // the other seat acts: sums over children
-            for (int k = 0; k < A; ++k) {
-                const F4 e = ld4(ecol + (size_t)k * ld);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) v.v[i] += e.v[i];
-            }
-            if (WITH_BR)
-                for (int k = 0; k < A; ++k) {
-                    const F4 e = ld4(evbr_p + (size_t)(fc + k) * ld + h0);
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) vbr.v[i] += e.v[i];
-                }
-        } else {
-            const int m = c.mode[p];
-            for (int k = 0; k < A; ++k) {
-                const F4 e = ld4(ecol + (size_t)k * ld);
-                const F4 s = strat4(c, m, fs + k, fs, A, h0);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) v.v[i] += s.v[i] * e.v[i];
-            }
-            if (WITH_BR) {
-                vbr = ld4(evbr_p + (size_t)fc * ld + h0);
-                for (int k = 1; k < A; ++k) {
-                    const F4 e = ld4(evbr_p + (size_t)(fc + k) * ld + h0);
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) vbr.v[i] = fmaxf(vbr.v[i], e.v[i]);
-                }
-            }
-            if (UPDATE && p == c.upd_p) {
-                float* rcol = c.B.regret + (size_t)fs * ld + h0;
-                float* scol = c.B.strat + (size_t)fs * ld + h0;
-                const float w = (float)(c.iter + 1);
-                F4 ssum = splat(0.0f);
-                for (int k = 0; k < A; ++k) {  // pass A: positive regret mass (new regrets are recomputed in pass B)
-                    const F4 e = ld4(ecol + (size_t)k * ld), rg = ld4(rcol + (size_t)k * ld);
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float d = e.v[i] - v.v[i];
-                        float r;
-                        if (c.algo == PRL_ALGO_CFR_PLUS) r = fmaxf(d + rg.v[i], 0.0f);
-                        else if (c.algo == PRL_ALGO_LINEAR) r = w * d + rg.v[i];
-                        else r = d + rg.v[i];
-                        ssum.v[i] += fmaxf(r, 0.0f);
-                    }
-                }
-                const float uni = 1.0f / (float)A;
-                F4 inv;
-#pragma unroll
-                for (int i = 0; i < 4; ++i) inv.v[i] = (ssum.v[i] > 0.0f) ? 1.0f / ssum.v[i] : 0.0f;
-                for (int k = 0; k < A; ++k) {  // pass B: store regrets and the regret-matching strategy
-                    const F4 e = ld4(ecol + (size_t)k * ld);
-                    F4 rg = ld4(rcol + (size_t)k * ld), st;
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float d = e.v[i] - v.v[i];
-                        float r;
-                        if (c.algo == PRL_ALGO_CFR_PLUS) r = fmaxf(d + rg.v[i], 0.0f);
-                        else if (c.algo == PRL_ALGO_LINEAR) r = w * d + rg.v[i];
-                        else r = d + rg.v[i];
-                        rg.v[i] = r;
-                        st.v[i] = (ssum.v[i] > 0.0f) ? fmaxf(r, 0.0f) * inv.v[i] : uni;
-                    }
-                    st4(rcol + (size_t)k * ld, rg);
-                    st4(scol + (size_t)k * ld, st);
-                }
-            }
-        }
-        st4(ev_p + (size_t)n * ld + h0, v);
-        if (WITH_BR) st4(evbr_p + (size_t)n * ld + h0, vbr);
-    }
-}
-
-// ---- v2 row kernels: one CTA per node (ceil(R / 4) threads rounded up to a warp), node structure from ONE 16-byte
-// record instead of a chain of dependent loads (parent -> first_child[parent] -> slot[...] -> rows)
-constexpr int kRowThreadsMax = 352;  // 1326 hands / 4 per thread = 332 -> 11 warps
-
-// node_rec2[n] = {parent, slot of n, first slot of the parent's children, kind(parent) | n_children(parent) << 8}
-template <bool UPDATE_AVG>
-__global__ void __launch_bounds__(kRowThreadsMax, 4) reach2_kernel_v2(const Ctx2 c) {
-    const int ld = c.T.ld, R = c.T.n_range;
-    const int n = c.lo + blockIdx.x;
-    const int h0 = 4 * threadIdx.x;
-    if (h0 >= R) return;
-    const size_t N = (size_t)c.T.n_nodes;
-    const int4 rec = reinterpret_cast<const int4*>(c.T.node_rec2)[n];
-    const int par = rec.x, slot = rec.y, fs = rec.z, pk = rec.w & 0xff, A = rec.w >> 8;
 #pragma unroll 1
     for (int q = 0; q < 2; ++q) {
         if (!(c.mask & (1 << q))) continue;
@@ -272,23 +159,7 @@ __global__ void __launch_bounds__(kRowThreadsMax, 4) reach2_kernel_v2(const Ctx2
                 const F4 s = strat4(c, c.mode[q], slot, fs, A, h0);
 #pragma unroll
                 for (int i = 0; i < 4; ++i) r.v[i] = s.v[i] * rp.v[i];
-                if (UPDATE_AVG && q == c.upd_p) {
-                    float* ap = (float*)c.B.avg + (size_t)slot * ld + h0;
-                    if (c.algo == PRL_ALGO_CFR_PLUS) {  // CFRPlus.py:65-87 (float table)
-                        if (c.iter >= c.delay) {
-                            F4 a = ld4(ap);
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) a.v[i] = c.m_old * a.v[i] + c.m_new * s.v[i];
-                            st4(ap, a);
-                        }
-                    } else {
-                        F4 a = ld4(ap);
-                        const float w = (c.algo == PRL_ALGO_LINEAR) ? (float)(c.iter + 1) : 1.0f;  // LinearCFR.py:56-61
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) a.v[i] = a.v[i] + r.v[i] * w;  // VanillaCFR.py:57-62
-                        st4(ap, a);
-                    }
-                }
+                if (UPDATE_AVG && q == c.upd_p) avg_update(c, (float*)c.B.avg + (size_t)slot * ld + h0, s, r);
             } else {
                 r = rp;
             }
@@ -297,8 +168,39 @@ __global__ void __launch_bounds__(kRowThreadsMax, 4) reach2_kernel_v2(const Ctx2
     }
 }
 
+// block x = child node n of the level, thread = four hands; structure through the parent -> first_child -> slot chain
+template <bool UPDATE_AVG>
+__global__ void __launch_bounds__(kVecThreads) reach2_kernel(const Ctx2 c) {
+    const int n = c.lo + blockIdx.x;
+    const int h0 = 4 * (blockIdx.y * blockDim.x + threadIdx.x);
+    if (h0 >= c.T.n_range) return;
+    const int par = c.T.parent[n];
+    int fs = 0, pk = 0, A = 0;  // a root has no parent to read
+    if (par >= 0) {
+        fs = c.T.slot[c.T.first_child[par]];
+        pk = c.T.kind[par];
+        A = c.T.n_children[par];
+    }
+    reach_rows<UPDATE_AVG>(c, n, h0, par, c.T.slot[n], fs, pk, A);
+}
+
+// ---- v2 row kernels: one CTA per node (ceil(R / 4) threads rounded up to a warp), node structure from ONE 16-byte
+// record instead of a chain of dependent loads (parent -> first_child[parent] -> slot[...] -> rows)
+constexpr int kRowThreadsMax = 352;  // 1326 hands / 4 per thread = 332 -> 11 warps
+
+// node_rec2[n] = {parent, slot of n, first slot of the parent's children, kind(parent) | n_children(parent) << 8}
+template <bool UPDATE_AVG>
+__global__ void __launch_bounds__(kRowThreadsMax, 4) reach2_kernel_v2(const Ctx2 c) {
+    const int n = c.lo + blockIdx.x;
+    const int h0 = 4 * threadIdx.x;
+    if (h0 >= c.T.n_range) return;
+    const int4 rec = reinterpret_cast<const int4*>(c.T.node_rec2)[n];
+    reach_rows<UPDATE_AVG>(c, n, h0, rec.x, rec.y, rec.z, rec.w & 0xff, rec.w >> 8);
+}
+
+// ------------------------------------------------------------------------------------------------ decision nodes (bottom-up)
 // regrets + regret matching of the seat's own node with the A child rows held in registers (each row is loaded once);
-// same operations in the same order as the loops of value2_kernel -> identical results
+// same operations in the same order as the loops of value_rows -> identical results
 template <int A>
 __device__ __forceinline__ F4 own_node_update(const Ctx2& c, int fs, int h0, const float* ecol) {
     const size_t ld = c.T.ld;
@@ -322,38 +224,25 @@ __device__ __forceinline__ F4 own_node_update(const Ctx2& c, int fs, int h0, con
     for (int k = 0; k < A; ++k) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-            const float d = e[k].v[i] - v.v[i];
-            float r;
-            if (c.algo == PRL_ALGO_CFR_PLUS) r = fmaxf(d + rg[k].v[i], 0.0f);
-            else if (c.algo == PRL_ALGO_LINEAR) r = w * d + rg[k].v[i];
-            else r = d + rg[k].v[i];
-            rg[k].v[i] = r;
-            ssum.v[i] += fmaxf(r, 0.0f);
+            rg[k].v[i] = regret_step(c.algo, e[k].v[i] - v.v[i], rg[k].v[i], w);
+            ssum.v[i] += fmaxf(rg[k].v[i], 0.0f);
         }
     }
-    const float uni = 1.0f / (float)A;
-    F4 inv;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) inv.v[i] = (ssum.v[i] > 0.0f) ? 1.0f / ssum.v[i] : 0.0f;
+    const RegretMatch rm(ssum, A);
 #pragma unroll
     for (int k = 0; k < A; ++k) {
-        F4 st;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) st.v[i] = (ssum.v[i] > 0.0f) ? fmaxf(rg[k].v[i], 0.0f) * inv.v[i] : uni;
         st4(rcol + (size_t)k * ld, rg[k]);
-        st4(scol + (size_t)k * ld, st);
+        st4(scol + (size_t)k * ld, rm(rg[k]));
     }
     return v;
 }
 
-// work_rec2[t] = {node, first child, first slot of the children, kind | n_children << 8} of work-list entry t
-template <bool WITH_BR, bool UPDATE>
-__global__ void __launch_bounds__(kRowThreadsMax, 3) value2_kernel_v2(const Ctx2 c) {
+// ValueFiller.py:80-93 + _CFRBase.py:146-185 + regret matching of decision node n for hands h0..h0+3, given its
+// structure: first child fc, first table row fs of the children, kind, fan-out A.  REG_ROWS: the updating seat's own
+// node with fan-out 2..4 takes the register-resident own_node_update
+template <bool WITH_BR, bool UPDATE, bool REG_ROWS>
+__device__ __forceinline__ void value_rows(const Ctx2& c, int n, int fc, int fs, int kind, int A, int h0) {
     const int ld = c.T.ld;
-    const int h0 = 4 * threadIdx.x;
-    if (h0 >= c.T.n_range) return;
-    const int4 rec = reinterpret_cast<const int4*>(c.T.work_rec2)[c.lo + blockIdx.x];
-    const int n = rec.x, fc = rec.y, fs = rec.z, kind = rec.w & 0xff, A = rec.w >> 8;
     const size_t N = (size_t)c.T.n_nodes;
 #pragma unroll 1
     for (int p = 0; p < 2; ++p) {
@@ -374,7 +263,7 @@ __global__ void __launch_bounds__(kRowThreadsMax, 3) value2_kernel_v2(const Ctx2
 #pragma unroll
                     for (int i = 0; i < 4; ++i) vbr.v[i] += e.v[i];
                 }
-        } else if (UPDATE && p == c.upd_p && A >= 2 && A <= 4 && c.mode[p] == PRL_STRAT_F32) {
+        } else if (REG_ROWS && UPDATE && p == c.upd_p && A >= 2 && A <= 4 && c.mode[p] == PRL_STRAT_F32) {
             if (A == 2) v = own_node_update<2>(c, fs, h0, ecol);
             else if (A == 3) v = own_node_update<3>(c, fs, h0, ecol);
             else v = own_node_update<4>(c, fs, h0, ecol);
@@ -394,48 +283,49 @@ __global__ void __launch_bounds__(kRowThreadsMax, 3) value2_kernel_v2(const Ctx2
                     for (int i = 0; i < 4; ++i) vbr.v[i] = fmaxf(vbr.v[i], e.v[i]);
                 }
             }
-            if (UPDATE && p == c.upd_p) {  // any other fan-out: rows re-read from L1 / L2
+            if (UPDATE && p == c.upd_p) {  // any fan-out: rows re-read from L1 / L2
                 float* rcol = c.B.regret + (size_t)fs * ld + h0;
                 float* scol = c.B.strat + (size_t)fs * ld + h0;
                 const float w = (float)(c.iter + 1);
                 F4 ssum = splat(0.0f);
-                for (int k = 0; k < A; ++k) {
+                for (int k = 0; k < A; ++k) {  // pass A: positive regret mass (new regrets are recomputed in pass B)
                     const F4 e = ld4(ecol + (size_t)k * ld), rg = ld4(rcol + (size_t)k * ld);
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float d = e.v[i] - v.v[i];
-                        float r;
-                        if (c.algo == PRL_ALGO_CFR_PLUS) r = fmaxf(d + rg.v[i], 0.0f);
-                        else if (c.algo == PRL_ALGO_LINEAR) r = w * d + rg.v[i];
-                        else r = d + rg.v[i];
-                        ssum.v[i] += fmaxf(r, 0.0f);
-                    }
+                    for (int i = 0; i < 4; ++i) ssum.v[i] += fmaxf(regret_step(c.algo, e.v[i] - v.v[i], rg.v[i], w), 0.0f);
                 }
-                const float uni = 1.0f / (float)A;
-                F4 inv;
-#pragma unroll
-                for (int i = 0; i < 4; ++i) inv.v[i] = (ssum.v[i] > 0.0f) ? 1.0f / ssum.v[i] : 0.0f;
-                for (int k = 0; k < A; ++k) {
+                const RegretMatch rm(ssum, A);
+                for (int k = 0; k < A; ++k) {  // pass B: store regrets and the regret-matching strategy
                     const F4 e = ld4(ecol + (size_t)k * ld);
-                    F4 rg = ld4(rcol + (size_t)k * ld), st;
+                    F4 rg = ld4(rcol + (size_t)k * ld);
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float d = e.v[i] - v.v[i];
-                        float r;
-                        if (c.algo == PRL_ALGO_CFR_PLUS) r = fmaxf(d + rg.v[i], 0.0f);
-                        else if (c.algo == PRL_ALGO_LINEAR) r = w * d + rg.v[i];
-                        else r = d + rg.v[i];
-                        rg.v[i] = r;
-                        st.v[i] = (ssum.v[i] > 0.0f) ? fmaxf(r, 0.0f) * inv.v[i] : uni;
-                    }
+                    for (int i = 0; i < 4; ++i) rg.v[i] = regret_step(c.algo, e.v[i] - v.v[i], rg.v[i], w);
                     st4(rcol + (size_t)k * ld, rg);
-                    st4(scol + (size_t)k * ld, st);
+                    st4(scol + (size_t)k * ld, rm(rg));
                 }
             }
         }
         st4(ev_p + (size_t)n * ld + h0, v);
         if (WITH_BR) st4(evbr_p + (size_t)n * ld + h0, vbr);
     }
+}
+
+// block x = work-list entry t -> decision node n, thread = four hands; structure through order / first_child / slot
+template <bool WITH_BR, bool UPDATE>
+__global__ void __launch_bounds__(kVecThreads) value2_kernel(const Ctx2 c) {
+    const int h0 = 4 * (blockIdx.y * blockDim.x + threadIdx.x);
+    if (h0 >= c.T.n_range) return;
+    const int n = c.T.order[c.lo + blockIdx.x];
+    const int kind = c.T.kind[n], fc = c.T.first_child[n], A = c.T.n_children[n];
+    value_rows<WITH_BR, UPDATE, false>(c, n, fc, c.T.slot[fc], kind, A, h0);
+}
+
+// work_rec2[t] = {node, first child, first slot of the children, kind | n_children << 8} of work-list entry t
+template <bool WITH_BR, bool UPDATE>
+__global__ void __launch_bounds__(kRowThreadsMax, 3) value2_kernel_v2(const Ctx2 c) {
+    const int h0 = 4 * threadIdx.x;
+    if (h0 >= c.T.n_range) return;
+    const int4 rec = reinterpret_cast<const int4*>(c.T.work_rec2)[c.lo + blockIdx.x];
+    value_rows<WITH_BR, UPDATE, true>(c, rec.x, rec.y, rec.z, rec.w & 0xff, rec.w >> 8, h0);
 }
 
 // ------------------------------------------------------------------------------------------------ chance nodes (bottom-up)
@@ -540,6 +430,111 @@ __device__ __forceinline__ float block_sum(float v, float* red /* >= 32 floats *
 //   - optional packed per-hand record (prl_tree_t.board_hand_rec): {gs, ge, 4 offsets into the card-row prefix array}
 //     in one 16-byte load instead of five narrow ones
 constexpr int kSegMax = 16;  // row entries per quad lane: ceil((n_deck - 1) / 4) <= 16
+constexpr int kSeg52 = 13;   // ceil((52 - 1) / 4): a 52-card deck, the only one terminal2_kernel_v3 is built for
+
+// ---- steps 2a, 2b and 3 of a showdown row over the CTA's shared arrays: ro[R] opponent reach row, srt[R + 1] reach in
+// strength order, rp[n_deck][kRowStride] card-row prefix sums
+// 2a. centred prefix sums of every card row in strength order: rp[c][i] = mass of the i weakest live hands holding card
+//     c, minus half the row's mass.  Quad lane qj scans entries [qj * seg, qj * seg + seg) in registers, seg <= SEG.
+template <int SEG>
+__device__ __forceinline__ void card_row_prefix(float* rp, const float* ro, const int16_t* row_order, int n_deck, int seg) {
+    const int row_len = n_deck - 1;
+    const int qj = threadIdx.x & 3;
+    for (int base = 0; base < n_deck; base += blockDim.x >> 2) {
+        const int cc = base + (threadIdx.x >> 2);
+        const bool live = cc < n_deck;
+        float inc[SEG];
+        float run = 0.0f;
+#pragma unroll
+        for (int i = 0; i < SEG; ++i) {
+            const int idx = qj * seg + i;
+            float v = 0.0f;
+            if (live && i < seg && idx < row_len) {
+                const int hh = row_order[cc * row_len + idx];
+                if (hh >= 0) v = ro[hh];
+            }
+            run += v;
+            inc[i] = run;
+        }
+        float sc = run;  // inclusive scan over the quad
+        float t = __shfl_up_sync(0xffffffffu, sc, 1, 4);
+        if (qj >= 1) sc += t;
+        t = __shfl_up_sync(0xffffffffu, sc, 2, 4);
+        if (qj >= 2) sc += t;
+        const float half = 0.5f * __shfl_sync(0xffffffffu, sc, 3, 4);
+        const float off = (sc - run) - half;
+        if (live) {
+            float* row = rp + cc * kRowStride;
+            if (qj == 0) row[0] = -half;
+#pragma unroll
+            for (int i = 0; i < SEG; ++i) {
+                const int idx = qj * seg + i;
+                if (i < seg && idx < row_len) row[idx + 1] = off + inc[i];
+            }
+        }
+    }
+}
+
+// 2b. centred exclusive prefix sums over srt[0..R], in place (each thread owns a contiguous segment, then a block scan;
+//     wsum holds the warp totals).  srt[] must be published before the call; it is published again on return.
+__device__ __forceinline__ void centred_scan(float* srt, float* wsum, int R) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, n_warps = blockDim.x >> 5;
+    const int per = (R + 1 + blockDim.x - 1) / blockDim.x;
+    const int i0 = threadIdx.x * per, i1 = min(R + 1, i0 + per);
+    float loc = 0.0f;
+    for (int i = i0; i < i1; ++i) loc += srt[i];
+    float incw = loc;  // inclusive scan of the per-thread sums within the warp
+    for (int o = 1; o < 32; o <<= 1) {
+        const float t = __shfl_up_sync(0xffffffffu, incw, o);
+        if (lane >= o) incw += t;
+    }
+    if (lane == 31) wsum[warp] = incw;
+    __syncthreads();
+    float before = 0.0f, total = 0.0f;  // every thread adds the warp totals itself (fixed order)
+    for (int w = 0; w < n_warps; ++w) {
+        const float x = wsum[w];
+        if (w < warp) before += x;
+        total += x;
+    }
+    float run = (incw - loc) + before - 0.5f * total;
+    for (int i = i0; i < i1; ++i) {
+        const float x = srt[i];
+        srt[i] = run;
+        run += x;
+    }
+    __syncthreads();
+}
+
+// 3. per hand: (weaker - stronger) mass over all live hands minus the same over the two card rows of the hand (the hands
+//    that share a card with it; the hand itself ties with itself and drops out), read through the packed hand records
+//    of the board
+template <bool WITH_BR>
+__device__ __forceinline__ void showdown_from_records(const uint4* rec, const float* srt, const float* rp, float scale, int R,
+                                                      float* ev_p, float* evbr_p) {
+    for (int h = threadIdx.x; h < R; h += blockDim.x) {
+        const uint4 q = rec[h];  // int16 x 8: gs, ge, c1 row + lt, c1 row + le, c2 row + lt, c2 row + le, 0, 0
+        const int gs = (int)(short)(q.x & 0xffffu);
+        float v = 0.0f;
+        if (gs >= 0) {
+            const float all = srt[gs] + srt[q.x >> 16];
+            const float rows = (rp[q.y & 0xffffu] + rp[q.y >> 16]) + (rp[q.z & 0xffffu] + rp[q.z >> 16]);
+            v = (all - rows) * scale;
+        }
+        ev_p[h] = v;
+        if (WITH_BR) evbr_p[h] = v;
+    }
+}
+
+// one CTA per terminal node; ValueFiller.py:34-62, 103-158 generalised (SURVEY.md appendix A)
+//
+// v2: same arithmetic with fewer instructions and barriers per terminal row
+//   - card rows are scanned by QUADS (4 lanes x <= 16 consecutive row entries, sequential in registers, then a 2-step
+//     quad scan) instead of one warp per row: 52 rows fit one pass of 208 threads
+//   - every prefix array is stored CENTRED,  E[i] = (mass of the i weakest) - total / 2,  so that
+//     (strictly weaker) - (strictly stronger) = E[gs] + E[ge]  without loading the totals
+//   - the scatter into strength order happens while the row is loaded; fold rows skip scans, showdown rows skip the sum
+//   - optional packed per-hand record (prl_tree_t.board_hand_rec): {gs, ge, 4 offsets into the card-row prefix array}
+//     in one 16-byte load instead of five narrow ones
 template <bool WITH_BR>
 __global__ void __launch_bounds__(kTermThreads) terminal2_kernel(const Ctx2 c) {
     extern __shared__ float smem[];
@@ -555,7 +550,6 @@ __global__ void __launch_bounds__(kTermThreads) terminal2_kernel(const Ctx2 c) {
     const size_t N = (size_t)c.T.n_nodes;
     const float scale = c.T.eq_const * c.T.pot[n] * 0.5f;
     const bool fold = kind == PRL_KIND_FOLD;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, n_warps = blockDim.x >> 5;
     const int row_len = n_deck - 1, seg = (row_len + 3) >> 2;
     const int qj = threadIdx.x & 3;
 #pragma unroll 1
@@ -612,83 +606,12 @@ __global__ void __launch_bounds__(kTermThreads) terminal2_kernel(const Ctx2 c) {
             if (ps >= 0) srt[ps] = r;
         }
         __syncthreads();
-        // 2a. centred prefix sums of every card row in strength order: rp[c][i] = mass of the i weakest live hands
-        //     holding card c, minus half the row's mass
-        for (int base = 0; base < n_deck; base += blockDim.x >> 2) {
-            const int cc = base + (threadIdx.x >> 2);
-            const bool live = cc < n_deck;
-            float inc[kSegMax];
-            float run = 0.0f;
-#pragma unroll
-            for (int i = 0; i < kSegMax; ++i) {
-                const int idx = qj * seg + i;
-                float v = 0.0f;
-                if (live && i < seg && idx < row_len) {
-                    const int hh = row_order[cc * row_len + idx];
-                    if (hh >= 0) v = ro[hh];
-                }
-                run += v;
-                inc[i] = run;
-            }
-            float sc = run;  // inclusive scan over the quad
-            float t = __shfl_up_sync(0xffffffffu, sc, 1, 4);
-            if (qj >= 1) sc += t;
-            t = __shfl_up_sync(0xffffffffu, sc, 2, 4);
-            if (qj >= 2) sc += t;
-            const float half = 0.5f * __shfl_sync(0xffffffffu, sc, 3, 4);
-            const float off = (sc - run) - half;
-            if (live) {
-                float* row = rp + cc * kRowStride;
-                if (qj == 0) row[0] = -half;
-#pragma unroll
-                for (int i = 0; i < kSegMax; ++i) {
-                    const int idx = qj * seg + i;
-                    if (i < seg && idx < row_len) row[idx + 1] = off + inc[i];
-                }
-            }
-        }
-        // 2b. centred exclusive prefix sums over srt[0..R] (each thread owns a contiguous segment, then a block scan)
-        const int per = (R + 1 + blockDim.x - 1) / blockDim.x;
-        const int i0 = threadIdx.x * per, i1 = min(R + 1, i0 + per);
-        float loc = 0.0f;
-        for (int i = i0; i < i1; ++i) loc += srt[i];
-        float incw = loc;  // inclusive scan of the per-thread sums within the warp
-        for (int o = 1; o < 32; o <<= 1) {
-            const float t = __shfl_up_sync(0xffffffffu, incw, o);
-            if (lane >= o) incw += t;
-        }
-        if (lane == 31) wsum[warp] = incw;
-        __syncthreads();
-        float before = 0.0f, total = 0.0f;  // every thread adds the warp totals itself (fixed order)
-        for (int w = 0; w < n_warps; ++w) {
-            const float x = wsum[w];
-            if (w < warp) before += x;
-            total += x;
-        }
-        float run = (incw - loc) + before - 0.5f * total;
-        for (int i = i0; i < i1; ++i) {
-            const float x = srt[i];
-            srt[i] = run;
-            run += x;
-        }
-        __syncthreads();
-        // 3. per hand: (weaker - stronger) mass over all live hands minus the same over the two card rows of the hand
-        //    (the hands that share a card with it; the hand itself ties with itself and drops out)
+        card_row_prefix<kSegMax>(rp, ro, row_order, n_deck, seg);
+        centred_scan(srt, wsum, R);
         if (c.T.board_hand_rec) {
-            const uint4* rec = reinterpret_cast<const uint4*>(c.T.board_hand_rec) + (size_t)b * R;
-            for (int h = threadIdx.x; h < R; h += blockDim.x) {
-                const uint4 q = rec[h];  // int16 x 8: gs, ge, c1 row + lt, c1 row + le, c2 row + lt, c2 row + le, 0, 0
-                const int gs = (int)(short)(q.x & 0xffffu);
-                float v = 0.0f;
-                if (gs >= 0) {
-                    const float all = srt[gs] + srt[q.x >> 16];
-                    const float rows = (rp[q.y & 0xffffu] + rp[q.y >> 16]) + (rp[q.z & 0xffffu] + rp[q.z >> 16]);
-                    v = (all - rows) * scale;
-                }
-                ev_p[h] = v;
-                if (WITH_BR) evbr_p[h] = v;
-            }
-        } else {
+            showdown_from_records<WITH_BR>(reinterpret_cast<const uint4*>(c.T.board_hand_rec) + (size_t)b * R, srt, rp,
+                                           scale, R, ev_p, evbr_p);
+        } else {  // 3. through the separate strength and card-row position tables
             const int16_t* gs_tab = c.T.board_gs + (size_t)b * R;
             const int16_t* ge_tab = c.T.board_ge + (size_t)b * R;
             const uchar4* row_pos = reinterpret_cast<const uchar4*>(c.T.board_row_pos) + (size_t)b * R;
@@ -712,10 +635,10 @@ __global__ void __launch_bounds__(kTermThreads) terminal2_kernel(const Ctx2 c) {
     }
 }
 
-// v3: the v2 arithmetic with every input of a showdown row STAGED IN SHARED MEMORY BY ASYNCHRONOUS COPIES (cp.async):
-// the opponent's reach row and the board's three tables (strength positions, card-row orders, packed hand records) are
-// requested together right after ONE structure load (work_rec2), so a terminal row pays two dependent global latencies
-// (record -> everything) instead of five (order -> node fields -> reach row -> row orders -> hand records).
+// v3: showdown rows only, with the v2 arithmetic and every input of a row STAGED IN SHARED MEMORY BY ASYNCHRONOUS COPIES
+// (cp.async): the opponent's reach row and the board's three tables (strength positions, card-row orders, packed hand
+// records) are requested together right after ONE structure load (work_rec2), so a terminal row pays two dependent global
+// latencies (record -> everything) instead of five (order -> node fields -> reach row -> row orders -> hand records).
 __device__ __forceinline__ void cp_async4(void* dst, const void* src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
 }
@@ -743,9 +666,11 @@ struct TermSmem {
     }
 };
 
-// work_rec2 entry of a TERMINAL work-list entry: {node, board id, pot (float bits), kind | (acted_last & 0xff) << 8}
-// SEG: card-row entries per quad lane held in registers - kSegMax (any deck) or the exact ceil((n_deck - 1) / 4)
-template <bool WITH_BR, int SEG>
+// work_rec2 entry of a TERMINAL work-list entry: {node, board id, pot (float bits), kind | (acted_last & 0xff) << 8}.
+// Fold rows come first among the terminals of a level and go to fold2_kernel; this kernel is launched on the showdown
+// rows after them, so its fold branch is never taken.  The branch stays: without it nvcc schedules the showdown path
+// differently, and the kernel measured 434 instead of 419 us per launch (hulh, 12 turns, H100 80GB HBM3 at 400 W).
+template <bool WITH_BR>
 __global__ void __launch_bounds__(kTermThreads) terminal2_kernel_v3(const Ctx2 c) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int R = c.T.n_range, ld = c.T.ld, n_deck = c.T.n_deck;
@@ -760,12 +685,11 @@ __global__ void __launch_bounds__(kTermThreads) terminal2_kernel_v3(const Ctx2 c
     float* rp = reinterpret_cast<float*>(smem_raw + L.rp);         // [n_deck][kRowStride]
     const int4 w = reinterpret_cast<const int4*>(c.T.work_rec2)[c.lo + blockIdx.x];
     const int n = w.x, b = w.y, kind = w.w & 0xff, acted_last = (w.w >> 8) & 0xff;
+    const bool fold = kind == PRL_KIND_FOLD;
+    const int qj = threadIdx.x & 3;
     const size_t N = (size_t)c.T.n_nodes;
     const float scale = c.T.eq_const * __int_as_float(w.z) * 0.5f;
-    const bool fold = kind == PRL_KIND_FOLD;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, n_warps = blockDim.x >> 5;
-    const int row_len = n_deck - 1, seg = (SEG == kSegMax) ? (row_len + 3) >> 2 : SEG;
-    const int qj = threadIdx.x & 3;
+    const int row_len = n_deck - 1;
     if (!fold) {  // the board's tables do not depend on the seat: requested once, consumed after the first wait
         const uint4* rec_g = reinterpret_cast<const uint4*>(c.T.board_hand_rec) + (size_t)b * R;
         for (int h = threadIdx.x; h < R; h += blockDim.x) cp_async16(rec_s + h, rec_g + h);
@@ -782,7 +706,7 @@ __global__ void __launch_bounds__(kTermThreads) terminal2_kernel_v3(const Ctx2 c
         float* ev_p = c.B.ev + ((size_t)p * N + n) * ld;
         float* evbr_p = WITH_BR ? c.B.ev_br + ((size_t)p * N + n) * ld : nullptr;
         __syncthreads();  // shared arrays are reused by the second seat
-        if (fold) {
+        if (fold) {  // not reached (see above)
             float part = 0.0f;
             for (int h = threadIdx.x; h < R; h += blockDim.x) {
                 const float r = ro_g[h];
@@ -794,8 +718,8 @@ __global__ void __launch_bounds__(kTermThreads) terminal2_kernel_v3(const Ctx2 c
                 const int cc = base + (threadIdx.x >> 2);
                 float run = 0.0f;
                 if (cc < n_deck) {
-                    for (int i = 0; i < seg; ++i) {
-                        const int idx = qj * seg + i;
+                    for (int i = 0; i < kSeg52; ++i) {
+                        const int idx = qj * kSeg52 + i;
                         if (idx < row_len) run += ro[pair_index(cc, idx + (idx >= cc), n_deck)];
                     }
                 }
@@ -815,7 +739,7 @@ __global__ void __launch_bounds__(kTermThreads) terminal2_kernel_v3(const Ctx2 c
             }
             continue;
         }
-        // ---- showdown: the reach row joins the outstanding table copies; 16-byte chunks, 4-byte tail
+        // the reach row joins the outstanding table copies; 16-byte chunks, 4-byte tail
         for (int i = threadIdx.x; i < R / 4; i += blockDim.x) cp_async16(ro + 4 * i, ro_g + 4 * i);
         for (int h = (R & ~3) + threadIdx.x; h < R; h += blockDim.x) cp_async4(ro + h, ro_g + h);
         for (int i = threadIdx.x; i <= R; i += blockDim.x) srt[i] = 0.0f;
@@ -826,79 +750,10 @@ __global__ void __launch_bounds__(kTermThreads) terminal2_kernel_v3(const Ctx2 c
             const int ps = pos_s[h];
             if (ps >= 0) srt[ps] = ro[h];
         }
-        // 2a. centred prefix sums of every card row (reads ro[] only: no barrier needed after the scatter yet)
-        for (int base = 0; base < n_deck; base += blockDim.x >> 2) {
-            const int cc = base + (threadIdx.x >> 2);
-            const bool live = cc < n_deck;
-            float inc[SEG];
-            float run = 0.0f;
-#pragma unroll
-            for (int i = 0; i < SEG; ++i) {
-                const int idx = qj * seg + i;
-                float v = 0.0f;
-                if (live && i < seg && idx < row_len) {
-                    const int hh = roword_s[cc * row_len + idx];
-                    if (hh >= 0) v = ro[hh];
-                }
-                run += v;
-                inc[i] = run;
-            }
-            float sc = run;  // inclusive scan over the quad
-            float t = __shfl_up_sync(0xffffffffu, sc, 1, 4);
-            if (qj >= 1) sc += t;
-            t = __shfl_up_sync(0xffffffffu, sc, 2, 4);
-            if (qj >= 2) sc += t;
-            const float half = 0.5f * __shfl_sync(0xffffffffu, sc, 3, 4);
-            const float off = (sc - run) - half;
-            if (live) {
-                float* row = rp + cc * kRowStride;
-                if (qj == 0) row[0] = -half;
-#pragma unroll
-                for (int i = 0; i < SEG; ++i) {
-                    const int idx = qj * seg + i;
-                    if (i < seg && idx < row_len) row[idx + 1] = off + inc[i];
-                }
-            }
-        }
+        card_row_prefix<kSeg52>(rp, ro, roword_s, n_deck, kSeg52);  // reads ro[] only: no barrier needed after the scatter yet
         __syncthreads();  // srt[] scattered
-        // 2b. centred exclusive prefix sums over srt[0..R]
-        const int per = (R + 1 + blockDim.x - 1) / blockDim.x;
-        const int i0 = threadIdx.x * per, i1 = min(R + 1, i0 + per);
-        float loc = 0.0f;
-        for (int i = i0; i < i1; ++i) loc += srt[i];
-        float incw = loc;
-        for (int o = 1; o < 32; o <<= 1) {
-            const float t = __shfl_up_sync(0xffffffffu, incw, o);
-            if (lane >= o) incw += t;
-        }
-        if (lane == 31) wsum[warp] = incw;
-        __syncthreads();
-        float before = 0.0f, total = 0.0f;
-        for (int k = 0; k < n_warps; ++k) {
-            const float x = wsum[k];
-            if (k < warp) before += x;
-            total += x;
-        }
-        float run = (incw - loc) + before - 0.5f * total;
-        for (int i = i0; i < i1; ++i) {
-            const float x = srt[i];
-            srt[i] = run;
-            run += x;
-        }
-        __syncthreads();
-        // 3. per hand
-        for (int h = threadIdx.x; h < R; h += blockDim.x) {
-            const uint4 q = rec_s[h];
-            const int gs = (int)(short)(q.x & 0xffffu);
-            float v = 0.0f;
-            if (gs >= 0) {
-                const float all = srt[gs] + srt[q.x >> 16];
-                const float rows = (rp[q.y & 0xffffu] + rp[q.y >> 16]) + (rp[q.z & 0xffffu] + rp[q.z >> 16]);
-                v = (all - rows) * scale;
-            }
-            ev_p[h] = v;
-            if (WITH_BR) evbr_p[h] = v;
-        }
+        centred_scan(srt, wsum, R);
+        showdown_from_records<WITH_BR>(rec_s, srt, rp, scale, R, ev_p, evbr_p);
     }
 }
 
@@ -1111,10 +966,10 @@ int value_levels2(Ctx2 c, bool with_br, bool update, int d_hi, int d_lo, int cha
     // terminal rows: fold rows and showdown rows in their own kernels (packed records, cp.async staging, 52-card decks); the
     // record-free kernel is the fallback for callers that pass NULL records or another deck size
     const bool packed = T.work_rec2 && T.board_hand_rec && !(T.n_range & 1) && T.level_nfold && T.n_deck <= 64 &&
-                        ((T.n_deck - 1 + 3) >> 2) == 13;
+                        ((T.n_deck - 1 + 3) >> 2) == kSeg52;
     const TermSmem tl(T.n_range, T.n_deck);
-    cudaFuncSetAttribute(terminal2_kernel_v3<true, 13>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tl.total);
-    cudaFuncSetAttribute(terminal2_kernel_v3<false, 13>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tl.total);
+    cudaFuncSetAttribute(terminal2_kernel_v3<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tl.total);
+    cudaFuncSetAttribute(terminal2_kernel_v3<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tl.total);
     int arr_mask = 0;
     for (int p = 0; p < 2; ++p)
         if (c.mask & (1 << p)) arr_mask |= (1 << (2 * p)) | (with_br ? (2 << (2 * p)) : 0);
@@ -1179,8 +1034,8 @@ int value_levels2(Ctx2 c, bool with_br, bool update, int d_hi, int d_lo, int cha
                 if (n_term > n_fold) {
                     c.lo = lo + n_nonterm + n_fold;
                     c.n = n_term - n_fold;
-                    if (with_br) terminal2_kernel_v3<true, 13><<<c.n, kTermThreads, tl.total, s>>>(c);
-                    else terminal2_kernel_v3<false, 13><<<c.n, kTermThreads, tl.total, s>>>(c);
+                    if (with_br) terminal2_kernel_v3<true><<<c.n, kTermThreads, tl.total, s>>>(c);
+                    else terminal2_kernel_v3<false><<<c.n, kTermThreads, tl.total, s>>>(c);
                     prl::count_launch();
                 }
             } else {

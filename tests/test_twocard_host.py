@@ -5,7 +5,7 @@ import numpy as np
 from pokerrl_b200.game import games, holdem_boards as hb
 from pokerrl_b200.game.flat_tree import enumerate_betting_tree
 from pokerrl_b200.game.hu_engine import HUBetting
-from twocard_common import fhp_tree, random_board_spec
+from twocard_common import fhp_tree, hulh_flop_subgame, nl_flop_subgame, random_board_spec
 
 
 def test_flop5holdem_betting_structure():
@@ -72,3 +72,26 @@ def test_structure_records_restate_the_pointer_chains():
         else:  # terminal entries carry what terminal2_kernel_v3 needs
             assert wrec[t, 1] == ft.board[n] and wrec[t, 3] >> 8 == (int(ft.acted_last[n]) & 0xff)
             assert wrec[t, 2:3].view(np.float32)[0] == np.float32(ft.pot[n])
+
+
+def test_work_order_puts_fold_rows_first_among_terminals():
+    """The value sweep launches fold2_kernel over the first level_nfold terminal entries of a level and
+    terminal2_kernel_v3 over the showdown entries after them, so v3 never meets a fold row: per level the work list must
+    be non-terminals, then every fold terminal, then showdowns, then all-in showdowns"""
+    from pokerrl_b200 import _native as nat
+    trees = [fhp_tree(random_board_spec(5, 3)), hulh_flop_subgame([[20, 21, 22], [30, 31]]), nl_flop_subgame()]
+    assert (trees[2].kind == nat.KIND_SHOWDOWN_ALLIN).any()
+    for ft in trees:
+        order, level_nonterm = ft.work_order()
+        for d in range(ft.n_levels):
+            lo, hi = int(ft.level_start[d]), int(ft.level_start[d + 1])
+            kinds = ft.kind[order[lo:hi]]
+            n_fold = int((ft.kind[lo:hi] == nat.KIND_FOLD).sum())  # DeviceTree's level_nfold[d]
+            n_show = int((kinds == nat.KIND_SHOWDOWN).sum())
+            n_allin = int((kinds == nat.KIND_SHOWDOWN_ALLIN).sum())
+            nt = int(level_nonterm[d])
+            assert nt + n_fold + n_show + n_allin == hi - lo
+            assert (kinds[:nt] <= nat.KIND_CHANCE).all()
+            assert (kinds[nt:nt + n_fold] == nat.KIND_FOLD).all()
+            assert (kinds[nt + n_fold:nt + n_fold + n_show] == nat.KIND_SHOWDOWN).all()
+            assert (kinds[nt + n_fold + n_show:] == nat.KIND_SHOWDOWN_ALLIN).all()
