@@ -28,8 +28,8 @@ typedef void* prl_stream_t; /* cudaStream_t */
 /* bumped whenever a struct below changes; prl_abi_version() returns the value the library was built with
    (2: prl_tree_t gained board_hand_rec / node_rec2 / work_rec2 / level_nfold; 3: board engine, legacy LUT natives;
     4: prl_board_sweep / prl_board_trunk take the algorithm; prl_tree_t gained the all-in terminals of two-card games: level_nallin / allin_nodes / allin_pot / allin_tiles /
-    allin_partial) */
-#define PRL_ABI_VERSION 4
+    allin_partial; 5: prl_board_update_cfrp / prl_board_avg_flush) */
+#define PRL_ABI_VERSION 5
 
 /* node kinds (game/_/tree/_/nodes.py:8-62 + ValueFiller.py:34-62) */
 enum {
@@ -279,6 +279,18 @@ int prl_board_build_tables(const int32_t* ranks, const uint64_t* board_mask, con
  * anyway; p1_only != 0 does nothing else (flush before the average strategy is evaluated or exported). */
 int prl_board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, int src_opp, const float* trunk_reach_opp,
                     int iter, int delay, int algo, float defer_w, int p1_only, prl_stream_t stream);
+
+/* CFR+ update sweep of seat p (prl_board_sweep with eval = 0, algo = PRL_ALGO_CFR_PLUS) that may move the averaging step
+ * (CFRPlus.py:65-87) of one iteration into the seat's next update sweep.  The step of iteration t averages in regret matching of
+ * the regrets the sweep of t writes; the seat's next sweep reads those regrets and matches them anyway, so it can apply the step
+ * to the average rows it loads and then apply its own - the same bits, one read and one write of the average for two steps.
+ * now = 1: this iteration's step (if iter >= delay) is written, now = 0: it is left pending and the sweep neither reads nor writes
+ * the average.  due = iteration of the seat's pending step, applied first (needs now = 1), or -1.  The caller keeps track of
+ * the pending step and calls prl_board_avg_flush before the average is read. */
+int prl_board_update_cfrp(const prl_board_game_t* g, int p, const float* trunk_reach_opp, int iter, int delay, int due, int now,
+                          prl_stream_t stream);
+/* applies seat p's pending CFR+ averaging step of iteration due on its own, from the seat's regret rows as they are */
+int prl_board_avg_flush(const prl_board_game_t* g, int p, int due, int delay, prl_stream_t stream);
 
 /* out[a][h] = 2^-frac_bits * sum over the n_sym suit permutations of w_total[a][perm(h)] (n_sym <= 1: no symmetrisation),
  * a < n_arr: the chance node's rows for the trunk sweep (after an all-reduce of w_total across GPUs, if sharded). */

@@ -79,6 +79,10 @@ class BoardCFRSolver:
         # Vanilla / Linear CFR: weight of the average-strategy contribution of each seat's last update that the post-deal rows
         # have not received yet (it is added by the next sweep that walks those rows: csrc/cfr_board.cu, DEFER)
         self._pending = [0.0, 0.0]
+        # CFR+: iteration of each seat's averaging step that is still pending (-1: none).  An update sweep with nothing pending
+        # leaves its step pending; the seat's next update sweep applies it together with its own (csrc/cfr_board.cu, AVG):
+        # every other sweep of a seat neither reads nor writes the average rows
+        self._avg_due = [-1, -1]
         self.game_cls, self.env_args = game_cls, env_args
         rules = game_cls.RULES
         spec = board_spec if board_spec is not None else BoardSpec.full_game(rules)
@@ -257,6 +261,13 @@ class BoardCFRSolver:
                  self.delay, nat.modes(*modes), 0, self.chance_level, _stream(self.device))
 
     def _sweep_begin(self, bufs, p, evaluate, src_own, src_opp):
+        if not evaluate and self.algo == nat.ALGO_CFR_PLUS:
+            t, due = self.iter_counter, self._avg_due[p]
+            now = 1 if due >= 0 or t < self.delay else 0  # an iteration before delay has no step to leave pending
+            self._avg_due[p] = -1 if now else t
+            nat.call("prl_board_update_cfrp", C.byref(self.g), p, self._trunk_reach_row(bufs, 1 - p), t, self.delay, due, now,
+                     _stream(self.device))
+            return
         defer_w = 0.0
         if not evaluate and self.algo != nat.ALGO_CFR_PLUS:  # this sweep walks the opponent's rows: its pending average goes in
             defer_w, self._pending[1 - p] = self._pending[1 - p], 0.0
@@ -264,9 +275,13 @@ class BoardCFRSolver:
                  self.iter_counter, self.delay, self.algo, defer_w, 0, _stream(self.device))
 
     def flush_average(self):
-        """Vanilla / Linear CFR: adds the average-strategy contributions that are still pending (a light P1-only sweep per seat)"""
+        """Applies the average-strategy updates that are still pending: CFR+ averaging steps (prl_board_avg_flush), Vanilla /
+        Linear CFR contributions (a light P1-only sweep per seat)"""
         with torch.cuda.device(self.device):
             for q in (0, 1):
+                if self._avg_due[q] >= 0:
+                    nat.call("prl_board_avg_flush", C.byref(self.g), q, self._avg_due[q], self.delay, _stream(self.device))
+                    self._avg_due[q] = -1
                 if self._pending[q] != 0.0:
                     nat.call("prl_board_sweep", C.byref(self.g), 1 - q, 0, 0, 0, self._trunk_reach_row(self.bufs, q),
                              self.iter_counter, self.delay, self.algo, self._pending[q], 1, _stream(self.device))
@@ -323,6 +338,7 @@ class BoardCFRSolver:
             for t in (self.regret, self.avg, self.bufs.regret, self.bufs.strat, self.bufs.avg):
                 t.zero_()
             self._pending = [0.0, 0.0]
+            self._avg_due = [-1, -1]
             self.modes = [nat.STRAT_UNIFORM64, nat.STRAT_UNIFORM64]
             self._reach_trunk(self.bufs, 3, -1, -1, self.modes)
 
@@ -364,8 +380,8 @@ class BoardCFRSolver:
         with torch.cuda.device(self.device):
             if self._eval_bufs is None:
                 self._eval_bufs = TreeBuffers(self.trunk, share=self.bufs)
+            self.flush_average()
             if self.algo != nat.ALGO_CFR_PLUS:  # normalised reach-weighted sums (LinearCFR.py:64-71, VanillaCFR.py:65-72)
-                self.flush_average()
                 modes, src = [nat.STRAT_AVG_SUM, nat.STRAT_AVG_SUM], SRC_AVG_SUM
             elif self.iter_counter == self.delay + 1:  # avg == copy of the current strategy (CFRPlus.py:83-84)
                 modes, src = [nat.STRAT_F32, nat.STRAT_F32], SRC_REGRET
@@ -404,6 +420,7 @@ class BoardCFRSolver:
     def load_natural_tables(self, ft, regret, avg):
         """inverse of natural_tables (teacher forcing in the parity tests, checkpoints written by the level engine)"""
         self._pending = [0.0, 0.0]  # the given average is complete
+        self._avg_due = [-1, -1]
         st = ft.board_subtree()
         dev = self.device
         src, dst = [], []
@@ -455,6 +472,7 @@ class BoardCFRSolver:
             raise ValueError("checkpoint table shape %s != %s" % (tuple(state["regret"].shape), tuple(self.regret.shape)))
         self.iter_counter, self.modes = int(state["iter_counter"]), list(state["modes"])
         self._pending = [0.0, 0.0]  # state_dict() flushes before it exports
+        self._avg_due = [-1, -1]
         self.regret.copy_(state["regret"])
         self.avg.copy_(state["avg"])
         self.bufs.regret.copy_(state["trunk_regret"])

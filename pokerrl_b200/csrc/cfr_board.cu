@@ -178,6 +178,8 @@ struct SweepArgs {
     const float* trunk_reach_opp;  // natural order row of the opponent's reach at the chance node
     int iter, delay;
     float m_old, m_new;            // CFRPlus.py:68-73
+    int pair;                      // CFR+ update: 1 = the seat's pending averaging step is applied before this iteration's
+    float m_old_due, m_new_due;    // the pending step's weights
     int src_own, src_opp;          // evaluation: 0 = regret matching of `regret`, 1 = `avg` rows as they are (CFR+ average),
                                    // 2 = `avg` rows normalised (reach-weighted sums of Vanilla / Linear CFR, LinearCFR.py:64-71)
     float rw;                      // weight of the instantaneous regret: 1, Linear CFR iter + 1 (LinearCFR.py:27-28)
@@ -242,6 +244,12 @@ __device__ __forceinline__ void node_strategy(const float (&g)[A], int src, floa
     for (int a = 0; a < A; ++a) s[a] = fmaf(s[a], inv, uni);
 }
 
+// one CFR+ averaging step (CFRPlus.py:65-87), avg = m_old * avg + m_new * s, rounded as nvcc contracted the plain expression
+// (FMUL of m_new * s, then FFMA): a step applied a sweep later or by the flush kernel gives the same bits
+__device__ __forceinline__ float avg_step(float m_old, float avg, float m_new, float s) {
+    return __fmaf_rn(m_old, avg, __fmul_rn(m_new, s));
+}
+
 __device__ __forceinline__ float ld_stream(const float* p) { return __ldcs(p); }
 __device__ __forceinline__ void st_stream(float* p, float v) { __stcs(p, v); }
 
@@ -255,9 +263,13 @@ __device__ __forceinline__ void st_stream(float* p, float v) { __stcs(p, v); }
 // new trunk reach, known only after this seat's trunk update.  The contribution of seat q's update is therefore added
 // during the NEXT sweep that walks q's rows anyway: P1 of the other seat's sweep computes exactly q's strategy and reach
 // at every node (defer_w = its weight).  P1ONLY: nothing but that (flush before an evaluation of the average strategy).
-template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false>
+// AVG (CFR+ update form): false = the average rows are neither read nor written - this iteration's averaging step, if any, is
+// left pending.  The strategy of the step of iteration t is regret matching of the regrets the sweep of t wrote, which the
+// seat's next sweep reads and matches for its value backup anyway: there (a.pair) the pending step is applied to the loaded
+// average right before this iteration's, one read and one write of the average rows for two steps.
+template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true>
 __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArgs a) {
-    static_assert(!(EVAL && DEFER) && (!P1ONLY || DEFER), "variants");
+    static_assert(!(EVAL && DEFER) && (!P1ONLY || DEFER) && (AVG || (!EVAL && !DEFER)), "variants");
     extern __shared__ __align__(128) unsigned char smem[];
     float* S = reinterpret_cast<float*>(smem + kSOff);
     float* Er = reinterpret_cast<float*>(smem + kErOff);
@@ -286,9 +298,10 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
     const float* tab_opp = (EVAL && a.src_opp >= 1) ? G.avg : G.regret;
     const float* tab_own = (EVAL && a.src_own >= 1) ? G.avg : G.regret;
     const int asis_opp = (EVAL && a.src_opp == 1) ? 1 : 0, asis_own = (EVAL && a.src_own == 1) ? 1 : 0;
-    const bool do_avg = !EVAL && !DEFER && a.iter >= a.delay;
+    const bool do_avg = !EVAL && !DEFER && AVG && a.iter >= a.delay;
+    const bool pair = do_avg && a.pair;
     const bool defer_now = DEFER && a.defer_w != 0.0f;
-    const bool read_avg = do_avg && a.m_old != 0.0f;
+    const bool read_avg = do_avg && (pair ? a.m_old_due : a.m_old) != 0.0f;  // the first step applied reads the stored average
 
     // private chance-sum accumulators of this CTA (global, L2-resident): [2][kRange] int64
     long long* wp = reinterpret_cast<long long*>(G.w_private) + (size_t)blockIdx.x * 2 * kRange;
@@ -587,7 +600,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
         __syncthreads();  // B4: prefix arrays complete
 
         // ------------------------------------------------------------------------------------------ P3: values, bottom-up
-        auto p3_hand = [&](int k, const float (&gown)[NOWN], const float (&av)[NOWN]) {
+        auto p3_hand = [&](int k, const float (&gown)[NOWN], float (&av)[NOWN]) {
             const int i = p3_pos(k);
             const uint64_t w = rec[i];
             const int hand = sh[i];
@@ -644,6 +657,10 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
 #pragma unroll
                         for (int c = 0; c < A; ++c) g[c] = gown[r0 + c];
                         node_strategy<A>(g, asis_own, s);
+                        if (pair) {  // s = the pending step's strategy: matching of the same regret rows, same statements
+#pragma unroll
+                            for (int c = 0; c < A; ++c) av[r0 + c] = avg_step(a.m_old_due, av[r0 + c], a.m_new_due, s[c]);
+                        }
                         float v = s[0] * e[fc];
 #pragma unroll
                         for (int c = 1; c < A; ++c) v += s[c] * e[fc + c];
@@ -665,7 +682,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
                             if (do_avg) {  // CFRPlus.py:65-87 (not reach-weighted)
 #pragma unroll
                                 for (int c = 0; c < A; ++c)
-                                    st_stream(avg_rows + (size_t)(r0 + c) * kLdb + i, a.m_old * av[r0 + c] + a.m_new * s[c]);
+                                    st_stream(avg_rows + (size_t)(r0 + c) * kLdb + i, avg_step(a.m_old, av[r0 + c], a.m_new, s[c]));
                             }
                         }
                     }
@@ -702,6 +719,33 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
     for (int h = tid; h < (EVAL ? 2 : 1) * kRange; h += kThreads) {
         const long long v = __ldcg(wp + h);  // L2: where the REDs landed
         if (v != 0) atomicAdd(wt + h, (unsigned long long)v);
+    }
+}
+
+// A pending CFR+ averaging step of seat P on its own (before the average is read or exported): the strategy from the seat's
+// regret rows, which no sweep has changed since the step's iteration, by the statements of board_sweep_kernel.  One CTA per
+// board; hands that hold a board card (positions >= kLive) are never written, as in the sweep.
+template <class SH, int P>
+__global__ void __launch_bounds__(256) avg_flush_kernel(float* __restrict__ regret, float* __restrict__ avg, float m_old, float m_new) {
+    constexpr size_t kBoardFloats = (size_t)SH::rows * kLdb;
+    const float* reg_b = regret + (size_t)blockIdx.x * kBoardFloats;
+    float* avg_b = avg + (size_t)blockIdx.x * kBoardFloats;
+    for (int i = threadIdx.x; i < kLive; i += blockDim.x) {
+        static_for<0, SH::N>([&](auto I) {
+            constexpr int n = decltype(I)::value;
+            if constexpr (SH::kind(n) == P) {
+                constexpr int A = SH::n_children(n), r0 = SH::row_of(SH::first_child(n));
+                float g[A], s[A];
+#pragma unroll
+                for (int c = 0; c < A; ++c) g[c] = ld_stream(reg_b + (size_t)(r0 + c) * kLdb + i);
+                node_strategy<A>(g, 0, s);
+#pragma unroll
+                for (int c = 0; c < A; ++c) {
+                    float* ap = avg_b + (size_t)(r0 + c) * kLdb + i;
+                    st_stream(ap, avg_step(m_old, (m_old != 0.0f) ? ld_stream(ap) : 0.0f, m_new, s[c]));
+                }
+            }
+        });
     }
 }
 
@@ -1024,14 +1068,22 @@ int default_grid() {
     return cached[dev];
 }
 
-template <int P, bool EVAL, bool DEFER = false, bool P1ONLY = false>
+template <int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true>
 int launch_sweep(const SweepArgs& a, int grid, cudaStream_t s) {
-    auto kern = board_sweep_kernel<ShapeFHP, P, EVAL, DEFER, P1ONLY>;
+    auto kern = board_sweep_kernel<ShapeFHP, P, EVAL, DEFER, P1ONLY, AVG>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);  // per device: set every time
     if (e != cudaSuccess) return prl::check(e, "prl_board_sweep: shared memory opt-in");
     kern<<<grid, kThreads, kSmemBytes, s>>>(a);
     prl::count_launch();
     return 0;
+}
+
+// CFRPlus.py:68-73: weights of the averaging step of iteration iter (the first one, iter == delay, copies the strategy)
+void cfrp_weights(int iter, int delay, float* m_old, float* m_new) {
+    const double cw = 0.5 * ((double)iter * (iter + 1) - (double)delay * (delay + 1));
+    const double nw = (double)iter - delay + 1;
+    *m_old = (iter > delay) ? (float)(cw / (cw + nw)) : 0.0f;
+    *m_new = (iter > delay) ? (float)(nw / (cw + nw)) : 1.0f;
 }
 
 }  // namespace
@@ -1066,8 +1118,10 @@ extern "C" int prl_board_build_tables(const int32_t* ranks, const uint64_t* boar
     return prl::check(cudaGetLastError(), "prl_board_build_tables");
 }
 
-extern "C" int prl_board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, int src_opp, const float* trunk_reach_opp,
-                               int iter, int delay, int algo, float defer_w, int p1_only, prl_stream_t stream) {
+// CFR+ update, averaging mode: due = iteration of the seat's pending averaging step (-1: none), now = 1: this iteration's step is
+// written, 0: it is left pending.  Today's form (-1, 1), deferred (-1, 0), paired (due, 1).
+static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, int src_opp, const float* trunk_reach_opp, int iter,
+                       int delay, int algo, float defer_w, int p1_only, int due, int now, prl_stream_t stream) {
     if (algo != PRL_ALGO_CFR_PLUS && algo != PRL_ALGO_VANILLA && algo != PRL_ALGO_LINEAR) return prl::fail("prl_board_sweep: bad algo");
     const bool defer = !eval && algo != PRL_ALGO_CFR_PLUS;
     if (p1_only && !defer) return prl::fail("prl_board_sweep: p1_only is the average flush of Vanilla / Linear CFR");
@@ -1077,6 +1131,9 @@ extern "C" int prl_board_sweep(const prl_board_game_t* g, int p, int eval, int s
     if (p < 0 || p > 1) return prl::fail("prl_board_sweep: bad seat");
     if (!g->tables || !g->regret || !g->avg || !g->w_private || !g->w_total || !trunk_reach_opp)
         return prl::fail("prl_board_sweep: missing buffers");
+    const bool step = now && iter >= delay;  // this iteration's averaging step is written
+    if (due != -1 && (due < delay || !step))
+        return prl::fail("prl_board_sweep: a pending averaging step (iteration >= delay) is written with this iteration's");
     cudaStream_t s = (cudaStream_t)stream;
     const int grid = g->grid > 0 ? g->grid : default_grid();
     SweepArgs a;
@@ -1084,10 +1141,10 @@ extern "C" int prl_board_sweep(const prl_board_game_t* g, int p, int eval, int s
     a.trunk_reach_opp = trunk_reach_opp;
     a.iter = iter;
     a.delay = delay;
-    const double cw = 0.5 * ((double)iter * (iter + 1) - (double)delay * (delay + 1));  // CFRPlus.py:68-73
-    const double nw = (double)iter - delay + 1;
-    a.m_old = (iter > delay) ? (float)(cw / (cw + nw)) : 0.0f;
-    a.m_new = (iter > delay) ? (float)(nw / (cw + nw)) : 1.0f;
+    cfrp_weights(iter, delay, &a.m_old, &a.m_new);
+    a.pair = due >= 0;
+    a.m_old_due = a.m_new_due = 0.0f;
+    if (a.pair) cfrp_weights(due, delay, &a.m_old_due, &a.m_new_due);
     a.src_own = src_own;
     a.src_opp = src_opp;
     a.rw = (algo == PRL_ALGO_LINEAR) ? (float)(iter + 1) : 1.0f;
@@ -1108,9 +1165,35 @@ extern "C" int prl_board_sweep(const prl_board_game_t* g, int p, int eval, int s
     int rc;
     if (eval) rc = (p == 0) ? launch_sweep<0, true>(a, grid, s) : launch_sweep<1, true>(a, grid, s);
     else if (defer) rc = (p == 0) ? launch_sweep<0, false, true>(a, grid, s) : launch_sweep<1, false, true>(a, grid, s);
-    else rc = (p == 0) ? launch_sweep<0, false>(a, grid, s) : launch_sweep<1, false>(a, grid, s);
+    else if (step) rc = (p == 0) ? launch_sweep<0, false>(a, grid, s) : launch_sweep<1, false>(a, grid, s);
+    else rc = (p == 0) ? launch_sweep<0, false, false, false, false>(a, grid, s) : launch_sweep<1, false, false, false, false>(a, grid, s);
     if (rc) return rc;
     return prl::check(cudaGetLastError(), "prl_board_sweep");
+}
+
+extern "C" int prl_board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, int src_opp, const float* trunk_reach_opp,
+                               int iter, int delay, int algo, float defer_w, int p1_only, prl_stream_t stream) {
+    return board_sweep(g, p, eval, src_own, src_opp, trunk_reach_opp, iter, delay, algo, defer_w, p1_only, -1, 1, stream);
+}
+
+extern "C" int prl_board_update_cfrp(const prl_board_game_t* g, int p, const float* trunk_reach_opp, int iter, int delay, int due,
+                                     int now, prl_stream_t stream) {
+    return board_sweep(g, p, 0, 0, 0, trunk_reach_opp, iter, delay, PRL_ALGO_CFR_PLUS, 0.0f, 0, due, now, stream);
+}
+
+extern "C" int prl_board_avg_flush(const prl_board_game_t* g, int p, int due, int delay, prl_stream_t stream) {
+    if (!g || !shape_matches(g) || !layout_matches(g)) return prl::fail("prl_board_avg_flush: not the compiled shape / layout");
+    if (p < 0 || p > 1) return prl::fail("prl_board_avg_flush: bad seat");
+    if (due < delay) return prl::fail("prl_board_avg_flush: no averaging step before iteration delay");
+    if (!g->regret || !g->avg) return prl::fail("prl_board_avg_flush: missing buffers");
+    if (g->n_boards <= 0) return 0;
+    float m_old, m_new;
+    cfrp_weights(due, delay, &m_old, &m_new);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (p == 0) avg_flush_kernel<ShapeFHP, 0><<<g->n_boards, 256, 0, s>>>(g->regret, g->avg, m_old, m_new);
+    else avg_flush_kernel<ShapeFHP, 1><<<g->n_boards, 256, 0, s>>>(g->regret, g->avg, m_old, m_new);
+    prl::count_launch();
+    return prl::check(cudaGetLastError(), "prl_board_avg_flush");
 }
 
 extern "C" int prl_board_collect(const prl_board_game_t* g, int n_arr, const int16_t* sym_perm, int n_sym, float* out, int ld,
@@ -1143,9 +1226,8 @@ extern "C" int prl_board_trunk(const prl_board_game_t* g, const prl_trunk_t* t, 
     for (int n = 0; n < t->n_nodes; ++n)
         if (t->kind[n] == PRL_KIND_SHOWDOWN || t->kind[n] == PRL_KIND_SHOWDOWN_ALLIN)
             return prl::fail("prl_board_trunk: showdowns before the deal are not supported");
-    const double cw = 0.5 * ((double)iter * (iter + 1) - (double)delay * (delay + 1));  // CFRPlus.py:68-73
-    const double nw = (double)iter - delay + 1;
-    const float m_old = (iter > delay) ? (float)(cw / (cw + nw)) : 0.0f, m_new = (iter > delay) ? (float)(nw / (cw + nw)) : 1.0f;
+    float m_old, m_new;
+    cfrp_weights(iter, delay, &m_old, &m_new);
     const double inv_scale = 1.0 / (double)(1ull << g->frac_bits);
     const long long* w = reinterpret_cast<const long long*>(g->w_total);
     if (peers && (n_peers < 1 || !w_scratch)) return prl::fail("prl_board_trunk: peer sum needs n_peers >= 1 and w_scratch");

@@ -1,14 +1,19 @@
 """Timing probe of the board engine on one GPU: python tools/board_probe.py [n_boards] [iterations] [grid]
-CUDA-event times of the update sweeps (per seat), the trunk part and the evaluation passes."""
+CUDA-event times of the iteration, of each form of the CFR+ update sweep and of the average flush (per launch, over many
+launches), and of the evaluation passes, with the bytes each form moves and the card it ran on."""
+import ctypes as C
 import json
 import os
+import statistics
+import subprocess
 import sys
 import time
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from pokerrl_b200.board_engine import BoardCFRSolver  # noqa: E402
+from pokerrl_b200 import _native as nat  # noqa: E402
+from pokerrl_b200.board_engine import BoardCFRSolver, _stream  # noqa: E402
 from pokerrl_b200.game import games  # noqa: E402
 from pokerrl_b200.game.holdem_boards import BoardSpec  # noqa: E402
 
@@ -34,26 +39,50 @@ s.iteration(iters)
 ev[1].record()
 torch.cuda.synchronize()
 it_ms = ev[0].elapsed_time(ev[1]) / iters
-# sweep kernel alone
-sw = []
-for rep in range(6):
-    for p in (0, 1):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        s._sweep_begin(s.bufs, p, False, 0, 0)
-        e1.record()
-        torch.cuda.synchronize()
-        sw.append(e0.elapsed_time(e1))
 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
 e0.record()
 a = s.exploitability_current()
 b = s.exploitability_average()
 e1.record()
 torch.cuda.synchronize()
-L = s.L
-bytes_sweep = s.n_boards * (35 * L["ldb"] * 4 + L["blob"])
-print(json.dumps({"boards": s.n_boards, "spec_s": t_spec, "build_s": t_build, "ms_per_iteration": it_ms,
-                  "iterations_per_s": 1e3 / it_ms, "sweep_ms": sorted(sw)[len(sw) // 2], "sweep_ms_all": sw,
-                  "sweep_GBps": bytes_sweep / (sorted(sw)[len(sw) // 2] * 1e-3) / 1e9, "bytes_per_sweep": bytes_sweep,
-                  "eval_both_ms": e0.elapsed_time(e1), "expl_cur": a, "expl_avg": b,
-                  "mem_GB": torch.cuda.max_memory_allocated() / 2 ** 30, "grid": s.g.grid}))
+eval_ms = e0.elapsed_time(e1)
+
+
+def per_launch_ms(launch, reps=10):
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        launch()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / reps
+
+
+# the forms of one seat's CFR+ update at iteration t (after this the solver's tables are no longer a CFR+ run)
+t, stream = s.iter_counter, _stream(s.device)
+forms = {
+    "defer": lambda p: nat.call("prl_board_update_cfrp", C.byref(s.g), p, s._trunk_reach_row(s.bufs, 1 - p), t, s.delay, -1, 0, stream),
+    "paired": lambda p: nat.call("prl_board_update_cfrp", C.byref(s.g), p, s._trunk_reach_row(s.bufs, 1 - p), t, s.delay, t - 1, 1,
+                                 stream),
+    "flush": lambda p: nat.call("prl_board_avg_flush", C.byref(s.g), p, t - 1, s.delay, stream),
+}
+row = s.L["ldb"] * 4
+bytes_per_board = {"defer": 21 * row + s.L["blob"], "paired": 35 * row + s.L["blob"], "flush": 21 * row}
+times = {k: [] for k in forms}
+for rnd in range(3):
+    for k, launch in forms.items():
+        for p in (0, 1):
+            times[k].append(per_launch_ms(lambda: launch(p)))
+res = {}
+for k in forms:
+    ms = statistics.median(times[k])
+    res[k] = {"ms": ms, "ms_all": times[k], "bytes": s.n_boards * bytes_per_board[k],
+              "GBps": s.n_boards * bytes_per_board[k] / (ms * 1e-3) / 1e9}
+try:
+    card = subprocess.check_output(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=name,power.limit,clocks.max.sm",
+                                    "--format=csv,noheader"], text=True).strip()
+except (OSError, subprocess.CalledProcessError):
+    card = torch.cuda.get_device_name() + " (power limit not readable)"
+print(json.dumps({"card": card, "boards": s.n_boards, "spec_s": t_spec, "build_s": t_build, "ms_per_iteration": it_ms,
+                  "iterations_per_s": 1e3 / it_ms, "update_sweep_forms": res, "eval_both_ms": eval_ms, "expl_cur": a,
+                  "expl_avg": b, "mem_GB": torch.cuda.max_memory_allocated() / 2 ** 30, "grid": s.g.grid}))
