@@ -59,6 +59,58 @@ def test_equity_matrix_and_dense_rows_on_reference_ranks():
     assert np.all(y[:, np.isin(hc, boards[0]).any(axis=1)] == y[:, np.isin(hc, boards[0]).any(axis=1)])  # finite
 
 
+@pytest.mark.parametrize("n_cols", [1, 16, 17, 33])
+@pytest.mark.parametrize("y2", ["none", "some"])
+def test_value_columns_in_chunks_of_16(n_cols, y2):
+    """prl_allin_values computes 16 columns per launch, all launches sharing one `partial` buffer: 1, 16, 17 and 33 columns
+    (an incomplete launch, one full launch, a last launch of one column, three launches) against float64 x E^T * scale at
+    1e-6.  The optional second output of a column (y2_rows, NULL as a whole or for some columns) is bit for bit y."""
+    import ctypes as C
+    import torch
+    from pokerrl_b200 import _native as nat
+    eq, E64, boards, hc = _golden_equity()
+    rng = np.random.default_rng(n_cols)
+    x = make_reach(100 + n_cols, np.repeat(boards[:1], n_cols, axis=0), hc).astype(np.float32)
+    x[rng.random(n_cols) < 0.2] *= 1e-4
+    scale = rng.uniform(0.5, 40.0, n_cols).astype(np.float32)
+    xt = torch.zeros(n_cols, 1328, dtype=torch.float32, device="cuda")
+    xt[:, :1326] = torch.from_numpy(x).cuda()
+    yt = torch.full((n_cols, 1328), float("nan"), dtype=torch.float32, device="cuda")
+    y2t = torch.full((n_cols, 1328), float("nan"), dtype=torch.float32, device="cuda")
+    given = [y2 == "some" and c % 3 != 1 for c in range(n_cols)]  # column 0 always has one when any are given
+    ptrs = C.c_void_p * n_cols
+    y2_rows = ptrs(*[y2t[c].data_ptr() if given[c] else None for c in range(n_cols)]) if y2 == "some" else None
+    nat.call("prl_allin_values", C.c_void_p(eq.tiles.data_ptr()), eq.R, ptrs(*[xt[c].data_ptr() for c in range(n_cols)]),
+             ptrs(*[yt[c].data_ptr() for c in range(n_cols)]), y2_rows, scale.ctypes.data_as(C.c_void_p), n_cols,
+             C.c_void_p(eq.partial.data_ptr()), C.c_void_p(torch.cuda.current_stream().cuda_stream))
+    y, y2v = yt.cpu().numpy()[:, :1326], y2t.cpu().numpy()[:, :1326]
+    want = (x.astype(np.float64) @ E64.T) * scale[:, None].astype(np.float64)
+    errs = [_rel(y[c], want[c]) for c in range(n_cols)]
+    print("all-in columns %d (y2 %s): worst relative error %.2e" % (n_cols, y2, max(errs)))
+    assert max(errs) <= TOL, errs
+    for c in range(n_cols):
+        if given[c]:
+            assert np.array_equal(y2v[c].view(np.int32), y[c].view(np.int32)), c
+        else:
+            assert np.isnan(y2v[c]).all(), c
+
+
+_EQ = []
+
+
+def _golden_equity():
+    """(AllinEquity, float64 E, boards, hand cards) of the golden boards with weights (b % 16 + 8) / 64, built once"""
+    if not _EQ:
+        from pokerrl_b200.allin import AllinEquity
+        rules = _rules()
+        hc = np.asarray(rules.get_lut_holder().LUT_IDX_2_HOLE_CARDS).astype(np.int64)
+        boards, ranks = GOLD["boards"], GOLD["ranks"]
+        w = (np.arange(len(boards)) % 16 + 8.0) / 64.0
+        eq = AllinEquity(rules, BoardSpec(boards, w, np.ones(len(boards)), None, "golden boards"))
+        _EQ.append((eq, o2.allin_equity_matrix(ranks, w, hc, 52), boards, hc))
+    return _EQ[0]
+
+
 def test_suit_symmetrised_matrix_equals_full_enumeration():
     """isomorphism classes + the 24 hand permutations give the matrix of the explicit board set (a deck subset keeps it small)"""
     import torch

@@ -42,10 +42,12 @@ def _assert_same(a, b):
         assert a.exploitability_average() == b.exploitability_average()
 
 
-@pytest.mark.parametrize("delay", [0, 2])
-def test_paired_averaging_equals_the_immediate_form(delay):
+@pytest.mark.parametrize("delay, grid", [pytest.param(d, 0, id=str(d)) for d in (0, 2)]
+                         + [pytest.param(d, 7, id="%d-grid7" % d) for d in (0, 2)])
+def test_paired_averaging_equals_the_immediate_form(delay, grid):
+    """grid 7: every CTA walks 3 or 4 of the 24 boards, so the defer and paired forms carry their state from board to board"""
     spec = random_board_spec(24, 41)
-    a, ref = _engine(spec, delay=delay), _engine(spec, immediate=True, delay=delay)
+    a, ref = _engine(spec, delay=delay, grid=grid), _engine(spec, immediate=True, delay=delay, grid=grid)
     for n in (1, 2, 3, 7):
         a.reset()
         ref.reset()
@@ -78,28 +80,33 @@ def test_interrupted_pairs_equal_an_uninterrupted_run():
 
 
 def test_shards_pair_like_one_device():
-    """two 'ranks' on one device against one rank holding every board, odd iteration count, after a flush"""
+    """two 'ranks' on one device against one rank holding every board, odd iteration count, after a flush; 3 boards give one
+    rank a single board, 1 board leaves one rank without any"""
     import torch
-    spec = random_board_spec(30, 44)
-    one = _engine(spec)
-    parts = [_engine(spec, rank=r, world=2, reduce_fn=lambda t: None) for r in range(2)]
-    for it in range(5):
-        one.iteration(1)
-        for p in (0, 1):
+    for n_boards in (30, 3, 1):
+        spec = random_board_spec(n_boards, 44)
+        one = _engine(spec)
+        parts = [_engine(spec, rank=r, world=2, reduce_fn=lambda t: None) for r in range(2)]
+        for it in range(5):
+            one.iteration(1)
+            for p in (0, 1):
+                for e in parts:
+                    e._update_begin(p)
+                tot = parts[0].w_total + parts[1].w_total
+                for e in parts:
+                    e.w_total.copy_(tot)
+                    e._update_end(p)
             for e in parts:
-                e._update_begin(p)
-            tot = parts[0].w_total + parts[1].w_total
-            for e in parts:
-                e.w_total.copy_(tot)
-                e._update_end(p)
-        for e in parts:
-            e.iter_counter += 1
-    for e in [one] + parts:
-        assert e._avg_due == [4, 4]
-        e.flush_average()
-    ldb, rpb = one.regret.shape[1], one.rows_per_board
-    for r, e in enumerate(parts):  # rank r holds boards r, r + 2, ...
-        assert torch.equal(e.regret.view(e.n_boards, rpb, ldb), one.regret.view(one.n_boards, rpb, ldb)[r::2])
-        assert torch.equal(e.avg.view(e.n_boards, rpb, ldb), one.avg.view(one.n_boards, rpb, ldb)[r::2])
-        assert torch.equal(e.bufs.regret, one.bufs.regret) and torch.equal(e.bufs.avg, one.bufs.avg)
-    assert np.count_nonzero(one.avg.cpu().numpy()) > 0
+                e.iter_counter += 1
+        for e in [one] + parts:
+            assert e._avg_due == [4, 4]
+            e.flush_average()
+        ldb, rpb = one.regret.shape[1], one.rows_per_board
+
+        def per_board(e, tab):  # a rank without boards keeps one placeholder row
+            return tab[:e.n_rows].view(e.n_boards, rpb, ldb)
+        for r, e in enumerate(parts):  # rank r holds boards r, r + 2, ...
+            assert torch.equal(per_board(e, e.regret), per_board(one, one.regret)[r::2])
+            assert torch.equal(per_board(e, e.avg), per_board(one, one.avg)[r::2])
+            assert torch.equal(e.bufs.regret, one.bufs.regret) and torch.equal(e.bufs.avg, one.bufs.avg)
+        assert np.count_nonzero(one.avg.cpu().numpy()) > 0

@@ -135,111 +135,131 @@ def _live_mask(ft, spec_boards):
     return ~blocked[np.maximum(ft.board[node_of_slot], 0)]
 
 
-@pytest.mark.parametrize("iso", [False, True])
-def test_teacher_forced_steps_match_float64_oracle(iso):
-    """Along an oracle run, every HALF-iteration starts from the oracle's tables: exploitability of the current / average
-    strategy under given tables, and the regrets / average after one seat's update from given tables, at 1e-6.
+def _with_grids(values, grids=(1, 7)):
+    """parameter sets (value, grid): the default grid (2 CTAs per SM: one board or none per CTA at these sizes) under the
+    value's own id, then one CTA and 7 CTAs, which loop over several boards each (7 divides none of the board counts here)"""
+    return ([pytest.param(v, 0, id=str(v)) for v in values]
+            + [pytest.param(v, g, id="%s-grid%d" % (v, g)) for g in grids for v in values])
+
+
+def _skewed(spec, seed=0):
+    """the boards of `spec` with unequal deal probabilities and multiplicities (sum of prob * mult = 1), so that a sweep that
+    weighted a board with another board's numbers could not pass"""
+    rng = np.random.default_rng(seed)
+    n = len(spec.boards)
+    mult = rng.uniform(0.5, 1.5, n)
+    prob = rng.uniform(0.5, 1.5, n)
+    prob /= (prob * mult).sum()
+    return BoardSpec(spec.boards, prob, mult, None, spec.note + ", skewed weights")
+
+
+def _teacher_forced(spec, algo="CFRPlus", grid=0, delay=0, warm=0, counters=range(4)):
+    """Along an oracle run (`warm` oracle iterations first), every HALF-iteration at the iteration counters `counters` starts
+    from the oracle's tables: exploitability of the current / average strategy under given tables, and the regrets / average
+    after one seat's update from given tables, at 1e-6.  Returns the errors per half-iteration.
     Why per seat and why masks: where all actions of a hand are worth exactly the same, the float64 oracle's regrets are
     +-1e-15 round-off and regret matching turns them into a pure strategy (SURVEY.md headline 5) - the next seat's values
     then depend on noise.  Regrets are continuous in the inputs; the average strategy is compared with the conditioning of
     regret matching taken out (the engine stores nothing for hands that hold a board card)."""
-    if iso:
-        from pokerrl_b200.game.games import FlopHoldemRules
-        spec = BoardSpec.full_game(FlopHoldemRules, isomorphic=True, deck_subset=[0, 1, 2, 3, 4, 5, 6, 7, 48, 49, 50, 51])
-    else:
-        spec = random_board_spec(48, 21)
+    from pokerrl_b200 import _native as nat
     ft = fhp_tree(spec)
-    orc = _oracle(ft, lean=True)
-    s = _engine(spec)
+    orc = _oracle(ft, algo, lean=True, delay=delay)
+    s = _engine(spec, algo=algo, grid=grid, delay=delay)
+    assert s.g.grid == (grid or nat.lib().prl_board_grid()) and s.delay == orc.delay == delay
+    orc.iteration(warm)
     live = _live_mask(ft, spec.boards)
     dec = np.nonzero((ft.kind <= 1) & (ft.first_child >= 0))[0]
     errs = []
-    for t in range(4):
+    for t in counters:
+        orc.iter_counter = t
         for p in (0, 1):
             s.load_natural_tables(ft, orc.regret, orc.avg)
             s.set_trunk_strategy_from_regrets()
-            s.iter_counter = orc.iter_counter
+            s.iter_counter = t
             e1 = e2 = 0.0
             if p == 0:
                 a, b = s.exploitability_current(), orc.exploitability_current()
                 e1 = abs(a - b) / abs(b)
-                if t > 0:
+                if t > delay:  # t == delay + 1: the average is the copy of the current strategy
                     a, b = s.exploitability_average(), orc.exploitability_average()
                     e2 = abs(a - b) / abs(b)
             s._update_begin(p)
             s._update_end(p)
             orc.half_iteration(p)
-            reg, avg = _natural(s, ft)
+            reg, avg = _natural(s, ft)  # flushes seat p's pending average step / contribution
             e3 = _rel(reg * live, orc.regret * live)
-            # average strategy of seat p's rows: sigma = r / sum(r) amplifies a regret error by max|r| / sum(r), so the
-            # difference is weighted by that condition number (rows whose regret sum reaches max|r| are held to 1e-6 as is)
             cond = np.zeros(orc.regret.shape)
-            for n in dec[ft.kind[dec] == p]:
-                fs, A = ft.first_slot[n], ft.n_children[n]
-                cond[fs:fs + A] = np.minimum(orc.regret[fs:fs + A].sum(axis=0) / np.abs(orc.regret).max(), 1.0)
-            e4 = float((np.abs(avg - orc.avg) * cond * live).max())
-            errs.append((e1, e2, e3, e4))
-            assert max(e1, e2, e3, e4) <= TOL, (t, p, e1, e2, e3, e4)
-        s.iter_counter += 1
-        orc.iter_counter += 1
-    print("teacher-forced relative errors (expl current, expl average, regrets, average) per half-iteration:",
-          ["%.1e %.1e %.1e %.1e" % e for e in errs])
-
-
-@pytest.mark.parametrize("algo", ["LinearCFR", "VanillaCFR"])
-def test_linear_and_vanilla_cfr_teacher_forced(algo):
-    """Vanilla / Linear CFR on the board engine (unclipped weighted regrets; the reach-weighted average sums of a seat are added
-    by the NEXT sweep over its rows or by flush_average): every half-iteration from the oracle's tables, regrets, average sums
-    and the exploitability of the current / the normalised average strategy at 1e-6."""
-    spec = random_board_spec(40, 17)
-    ft = fhp_tree(spec)
-    orc = _oracle(ft, algo, lean=True)
-    s = _engine(spec, algo=algo)
-    live = _live_mask(ft, spec.boards)
-    dec = np.nonzero((ft.kind <= 1) & (ft.first_child >= 0))[0]
-    errs = []
-    for t in range(4):
-        for p in (0, 1):
-            s.load_natural_tables(ft, orc.regret, orc.avg)
-            s.set_trunk_strategy_from_regrets()
-            s.iter_counter = orc.iter_counter
-            e1 = e2 = 0.0
-            if p == 0:
-                a, b = s.exploitability_current(), orc.exploitability_current()
-                e1 = abs(a - b) / abs(b)
-                if t > 0:
-                    a, b = s.exploitability_average(), orc.exploitability_average()
-                    e2 = abs(a - b) / abs(b)
-            s._update_begin(p)
-            s._update_end(p)
-            orc.half_iteration(p)
-            reg, avg = _natural(s, ft)  # flushes seat p's pending average contribution
-            e3 = _rel(reg * live, orc.regret * live)
-            # the sums take in sigma = r+ / sum(r+) of the UPDATED regrets, which amplifies a regret error by max|r| / sum(r+)
-            # (a hand whose actions tie has regrets of round-off size and a strategy decided by it): weighted by that
-            # condition number like the CFR+ average above; the unweighted difference is printed as well
-            # ... and the seat's reach at a node is the product of its strategies above it (trunk included), so a node's
-            # weight is the product of the condition numbers along its path
-            rp = np.maximum(orc.regret, 0.0)
-            cond = np.zeros(orc.regret.shape)
-            node_cond = {}
-            for n in dec[ft.kind[dec] == p]:  # ascending ids: ancestors first
-                fs, A = ft.first_slot[n], ft.n_children[n]
-                c = np.minimum(rp[fs:fs + A].sum(axis=0) / np.abs(orc.regret).max(), 1.0)
-                a = ft.parent[n]
-                while a >= 0 and a not in node_cond:
-                    a = ft.parent[a]
-                node_cond[n] = c * (node_cond[a] if a >= 0 else 1.0)
-                cond[fs:fs + A] = node_cond[n]
-            scale = max(np.abs(orc.avg).max(), 1e-300)
+            if algo == "CFRPlus":
+                # average strategy of seat p's rows: sigma = r / sum(r) amplifies a regret error by max|r| / sum(r), so the
+                # difference is weighted by that condition number (rows whose regret sum reaches max|r| are held to 1e-6 as is)
+                for n in dec[ft.kind[dec] == p]:
+                    fs, A = ft.first_slot[n], ft.n_children[n]
+                    cond[fs:fs + A] = np.minimum(orc.regret[fs:fs + A].sum(axis=0) / np.abs(orc.regret).max(), 1.0)
+                scale = 1.0
+            else:
+                # the sums take in sigma = r+ / sum(r+) of the UPDATED regrets, which amplifies a regret error by
+                # max|r| / sum(r+) (a hand whose actions tie has regrets of round-off size and a strategy decided by it):
+                # weighted by that condition number like the CFR+ average; the unweighted difference is returned as well
+                # ... and the seat's reach at a node is the product of its strategies above it (trunk included), so a node's
+                # weight is the product of the condition numbers along its path
+                rp = np.maximum(orc.regret, 0.0)
+                node_cond = {}
+                for n in dec[ft.kind[dec] == p]:  # ascending ids: ancestors first
+                    fs, A = ft.first_slot[n], ft.n_children[n]
+                    c = np.minimum(rp[fs:fs + A].sum(axis=0) / np.abs(orc.regret).max(), 1.0)
+                    a = ft.parent[n]
+                    while a >= 0 and a not in node_cond:
+                        a = ft.parent[a]
+                    node_cond[n] = c * (node_cond[a] if a >= 0 else 1.0)
+                    cond[fs:fs + A] = node_cond[n]
+                scale = max(np.abs(orc.avg).max(), 1e-300)
             e4 = float((np.abs(avg - orc.avg) * cond * live).max() / scale)
             e5 = _rel(avg * live, orc.avg * live)
             errs.append((e1, e2, e3, e4, e5))
-            assert max(e1, e2, e3, e4) <= TOL, (algo, t, p, e1, e2, e3, e4, e5)
-        s.iter_counter += 1
-        orc.iter_counter += 1
-    print(algo, "teacher-forced relative errors (expl current, expl average, regrets, average sums conditioned / raw) per "
+            assert max(e1, e2, e3, e4) <= TOL, (algo, grid, t, p, e1, e2, e3, e4, e5)
+    return errs
+
+
+def _print_errs(what, errs):
+    print(what, "teacher-forced relative errors (expl current, expl average, regrets, average conditioned / raw) per "
           "half-iteration:", ["%.1e %.1e %.1e %.1e %.1e" % e for e in errs])
+
+
+def _iso_spec():
+    from pokerrl_b200.game.games import FlopHoldemRules
+    return BoardSpec.full_game(FlopHoldemRules, isomorphic=True, deck_subset=[0, 1, 2, 3, 4, 5, 6, 7, 48, 49, 50, 51])
+
+
+@pytest.mark.parametrize("iso, grid", _with_grids([False, True]))
+def test_teacher_forced_steps_match_float64_oracle(iso, grid):
+    """CFR+ along an oracle run from the start (iterations 0 .. 3), 48 random boards or the 57 suit classes of a 12-card deck"""
+    spec = _iso_spec() if iso else _skewed(random_board_spec(48, 21))
+    _print_errs("CFRPlus grid %d" % grid, _teacher_forced(spec, grid=grid))
+
+
+@pytest.mark.parametrize("algo, grid", _with_grids(["LinearCFR", "VanillaCFR"]))
+def test_linear_and_vanilla_cfr_teacher_forced(algo, grid):
+    """Vanilla / Linear CFR on the board engine (unclipped weighted regrets; the reach-weighted average sums of a seat are added
+    by the NEXT sweep over its rows or by flush_average): every half-iteration from the oracle's tables, regrets, average sums
+    and the exploitability of the current / the normalised average strategy at 1e-6."""
+    _print_errs("%s grid %d" % (algo, grid), _teacher_forced(_skewed(random_board_spec(40, 17)), algo, grid=grid))
+
+
+@pytest.mark.parametrize("grid", [0, 7])
+def test_cfr_plus_delay_teacher_forced(grid):
+    """CFR+ with delay 2 at iteration counters 1 (no averaging step), 2 (the step copies the strategy), 3 (the first mixed
+    step; the average's exploitability is that of the current strategy) and 4: the `iter >= delay` gates and the weights
+    m_old / m_new with their delay offset, against the float64 oracle run with the same delay"""
+    _print_errs("CFRPlus delay 2 grid %d" % grid, _teacher_forced(_skewed(random_board_spec(37, 5)), grid=grid, delay=2, warm=1,
+                                                                  counters=range(1, 5)))
+
+
+@pytest.mark.parametrize("algo", ["CFRPlus", "LinearCFR", "VanillaCFR"])
+def test_teacher_forced_steps_late_in_a_run(algo):
+    """tables of 3 oracle iterations, then half-iterations at iteration counters 997 and 998: CFR+'s m_old / m_new close to 1
+    and Linear CFR's weight iter + 1 in the sweep, the trunk and the pending average contribution, far from 0"""
+    _print_errs("%s at iteration 997" % algo, _teacher_forced(_skewed(random_board_spec(37, 5)), algo, grid=7, warm=3,
+                                                              counters=(997, 998)))
 
 
 @pytest.mark.parametrize("algo", ["LinearCFR", "VanillaCFR"])
@@ -286,44 +306,58 @@ def test_free_running_trajectory_and_level_engine():
 
 
 def test_fixed_point_sums_do_not_depend_on_the_grid():
-    """the chance-node sums are integers: any number of CTAs (and, by the same argument, of GPUs) gives the same bits"""
-    spec = random_board_spec(64, 33)
-    runs = []
-    for grid in (0, 7, 64):
-        s = _engine(spec, grid=grid)
-        s.iteration(3)
-        runs.append((s.regret.clone(), s.bufs.regret.clone(), s.exploitability_current(), s.exploitability_average()))
+    """the chance-node sums are integers: any number of CTAs (and, by the same argument, of GPUs) gives the same bits - for
+    every algorithm, and for the average after a flush (Vanilla / Linear CFR: the P1-only flush sweep, then the evaluation
+    of the normalised sums)"""
     import torch
-    for r in runs[1:]:
-        assert torch.equal(r[0], runs[0][0]) and torch.equal(r[1], runs[0][1]) and r[2:] == runs[0][2:]
+    spec = _skewed(random_board_spec(64, 33))
+    for algo in ("CFRPlus", "LinearCFR", "VanillaCFR"):
+        runs = []
+        for grid in (0, 1, 7, 64):
+            s = _engine(spec, algo=algo, grid=grid)
+            s.iteration(3)
+            cur = s.exploitability_current()
+            s.flush_average()
+            runs.append((s.regret.clone(), s.bufs.regret.clone(), s.avg.clone(), s.bufs.avg.clone(), cur,
+                         s.exploitability_average()))
+        assert np.count_nonzero(runs[0][2].cpu().numpy()) > 0
+        for grid, r in zip((1, 7, 64), runs[1:]):
+            assert all(torch.equal(x, y) for x, y in zip(r[:4], runs[0][:4])) and r[4:] == runs[0][4:], (algo, grid)
+
+
+def _per_board(e, tab):
+    """[n_boards, rows_per_board, ldb] view of a post-deal table (a rank without boards keeps one placeholder row)"""
+    return tab[:e.n_rows].view(e.n_boards, e.rows_per_board, tab.shape[1])
 
 
 def test_shards_reproduce_the_single_device_run_bit_for_bit():
     """two 'ranks' on one device (boards round-robin), driven in lockstep with their integer sums added by hand in place of
-    the all-reduce, against one rank holding every board: identical tables, identical exploitability"""
+    the all-reduce, against one rank holding every board: identical tables, identical exploitability.  3 boards give one
+    rank a single board, 1 board leaves one rank without any."""
     import torch
-    spec = random_board_spec(30, 8)
-    one = _engine(spec)
-    parts = [_engine(spec, rank=r, world=2, reduce_fn=lambda t: None) for r in range(2)]
-    for it in range(3):
-        one.iteration(1)
-        for p in (0, 1):
+    for n_boards in (30, 3, 1):
+        spec = random_board_spec(n_boards, 8)
+        one = _engine(spec)
+        parts = [_engine(spec, rank=r, world=2, reduce_fn=lambda t: None) for r in range(2)]
+        assert [e.n_boards for e in parts] == [(n_boards + 1) // 2, n_boards // 2]
+        for it in range(3):
+            one.iteration(1)
+            for p in (0, 1):
+                for e in parts:
+                    e._update_begin(p)
+                tot = parts[0].w_total + parts[1].w_total
+                for e in parts:
+                    e.w_total.copy_(tot)
+                    e._update_end(p)
             for e in parts:
-                e._update_begin(p)
-            tot = parts[0].w_total + parts[1].w_total
-            for e in parts:
-                e.w_total.copy_(tot)
-                e._update_end(p)
+                e.iter_counter += 1
+        one.flush_average()
+        for r, e in enumerate(parts):  # rank r holds boards r, r + 2, ...
+            e.flush_average()
+            assert torch.equal(_per_board(e, e.regret), _per_board(one, one.regret)[r::2])
+            assert torch.equal(_per_board(e, e.avg), _per_board(one, one.avg)[r::2])
         for e in parts:
-            e.iter_counter += 1
-    ldb, rpb = one.regret.shape[1], one.rows_per_board
-    full = one.regret.view(one.n_boards, rpb, ldb)
-    full_avg = one.avg.view(one.n_boards, rpb, ldb)
-    for r, e in enumerate(parts):  # rank r holds boards r, r + 2, ...
-        assert torch.equal(e.regret.view(e.n_boards, rpb, ldb), full[r::2])
-        assert torch.equal(e.avg.view(e.n_boards, rpb, ldb), full_avg[r::2])
-    for e in parts:
-        assert torch.equal(e.bufs.regret, one.bufs.regret) and torch.equal(e.bufs.avg, one.bufs.avg)
+            assert torch.equal(e.bufs.regret, one.bufs.regret) and torch.equal(e.bufs.avg, one.bufs.avg)
 
 
 def test_single_launch_trunk_equals_the_level_kernel_trunk(monkeypatch):
