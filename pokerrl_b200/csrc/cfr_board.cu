@@ -68,6 +68,13 @@ static_assert(kBlobA % 16 == 0 && kRowIdxBytes % 16 == 0, "bulk copies move mult
 #ifndef PRL_BV_NEWTON
 #define PRL_BV_NEWTON 1      // regret matching: Newton step after MUFU.RCP (<= 1 ulp); 0 = the approximation as is (2^-23 relative)
 #endif
+#ifndef PRL_BV_PF
+#define PRL_BV_PF 1          // table rows into L2, update forms: 1 = each stream one phase ahead of its first use (own rows at B1
+                             // of their unit, the next unit's opponent rows at B2); 0 = all rows of the next board at the unit's top
+#endif
+#ifndef PRL_BV_STAMPS
+#define PRL_BV_STAMPS 0      // 1 = phase stamps: clock64() at the unit start and B1-B5 of sampled units (tools/board_phases.py)
+#endif
 constexpr int kVP1Pipe = PRL_BV_P1PIPE;
 constexpr bool kVRed = PRL_BV_RED, kVFoldLin = PRL_BV_FOLDLIN, kVErT = PRL_BV_ERT;
 // tried and removed: five-warp / one-warp-per-vector scans, the single-warp stage spread
@@ -216,6 +223,28 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// ---- phase stamps (PRL_BV_STAMPS builds only): thread 0 of CTA b < kStampCtas records, for its units it = 0, kStampEvery,
+//      2 kStampEvery, ... (kStampUnits of them), clock64() at the unit start (slot 0) and right after B1 .. B5 (slots 1-5), the
+//      SM id (slot 6) and it (slot 7).  prl_board_stamps copies the records out and clears them.
+#if PRL_BV_STAMPS
+constexpr int kStampCtas = 512, kStampUnits = 16, kStampEvery = 32, kStampSlots = 8;
+__device__ long long g_stamps[kStampCtas * kStampUnits * kStampSlots];
+#endif
+__device__ __forceinline__ void stamp(int it, int slot) {
+#if PRL_BV_STAMPS
+    if (threadIdx.x == 0 && blockIdx.x < kStampCtas && it % kStampEvery == 0 && it / kStampEvery < kStampUnits) {
+        long long* r = g_stamps + ((size_t)blockIdx.x * kStampUnits + it / kStampEvery) * kStampSlots;
+        r[slot] = clock64();
+        if (slot == 0) {
+            unsigned smid;
+            asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+            r[6] = smid;
+            r[7] = it;
+        }
+    }
+#endif
+}
+
 // strategy of one decision node from its table rows: regret matching (CFRPlus.py:43-63; the regrets of Vanilla / Linear
 // CFR are clipped first, LinearCFR.py:33-51) or the rows as they are (CFR+ average strategy)
 template <int A>
@@ -323,6 +352,21 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
         if (read_avg) bulk_prefetch_l2(G.avg + (size_t)jj * kBoardFloats + (size_t)OWN0 * kLdb, NOWN * kLdb * 4);
         if (defer_now) bulk_prefetch_l2(G.avg + (size_t)jj * kBoardFloats + (size_t)OPP0 * kLdb, NOPP * kLdb * 4);
     };
+    // Update forms (PRL_BV_PF): each stream one phase ahead of its first use, so that a CTA holds about one board's rows in L2,
+    // not two - two boards of the paired form (264 CTAs x (2 x 91 KB read + 61 KB stored)) overflow the 50 MB L2 of an H100,
+    // and rows evicted before their use are fetched twice.  The evaluation form stores nothing and fits two boards deep
+    // (31 MB): it keeps the whole-unit lead (measured: the phase schedule slowed it by 4 %).
+    constexpr bool kPfPhase = PRL_BV_PF && !EVAL;
+    // rows first read in P1: the next unit's opponent rows (DEFER: and the opponent's average rows), prefetched at B2 ...
+    auto prefetch_opp = [&](int jj) {
+        bulk_prefetch_l2(tab_opp + (size_t)jj * kBoardFloats + (size_t)OPP0 * kLdb, NOPP * kLdb * 4);
+        if (defer_now) bulk_prefetch_l2(G.avg + (size_t)jj * kBoardFloats + (size_t)OPP0 * kLdb, NOPP * kLdb * 4);
+    };
+    // ... rows first read in P3: this unit's own rows (paired form: and the average rows), prefetched at B1 to load behind P2
+    auto prefetch_own = [&](int jj) {
+        bulk_prefetch_l2(tab_own + (size_t)jj * kBoardFloats + (size_t)OWN0 * kLdb, NOWN * kLdb * 4);
+        if (read_avg) bulk_prefetch_l2(G.avg + (size_t)jj * kBoardFloats + (size_t)OWN0 * kLdb, NOWN * kLdb * 4);
+    };
     if (tid == 0 && j < nb) {  // first board's tables
         mbar_expect_tx(&bars[0], kBlobA);
         bulk_g2s(smem + kBlobOff, blob_g + (size_t)j * kBlobBytes, kBlobA, &bars[0]);
@@ -330,7 +374,8 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
             mbar_expect_tx(&bars[2], kRowIdxBytes);
             bulk_g2s(smem + kRowIdxOff, blob_g + (size_t)j * kBlobBytes + kBlobA, kRowIdxBytes, &bars[2]);
         }
-        prefetch_rows(j);
+        if constexpr (kPfPhase) prefetch_opp(j);
+        else prefetch_rows(j);
     }
 
     // P1 inputs of the thread's three strength positions (opponent rows + trunk reach).  kVP1Pipe: only the first position
@@ -357,10 +402,11 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
         const uint64_t* rec = reinterpret_cast<const uint64_t*>(blob);
         const int16_t* sh = reinterpret_cast<const int16_t*>(blob + kRecBytes);
         const int jn = j + gridDim.x;
+        stamp(it, 0);
         if (tid == 0 && jn < nb) {  // next board: records + hand ids into the other buffer (free since the last barrier), rows into L2
             mbar_expect_tx(&bars[buf ^ 1], kBlobA);
             bulk_g2s(smem + kBlobOff + (buf ^ 1) * kBlobA, blob_g + (size_t)jn * kBlobBytes, kBlobA, &bars[buf ^ 1]);
-            prefetch_rows(jn);
+            if constexpr (!kPfPhase) prefetch_rows(jn);
         }
         const float prob = __ldg(G.board_prob + j);
         if (it == 0) {
@@ -423,6 +469,14 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
             for (int k = 0; k < kPerThread; ++k) p1_hand(k, p1_g[k], p1_x0[k]);
         }
         __syncthreads();  // B1: S complete
+        stamp(it, 1);
+        if (kPfPhase && tid == 0) {
+            if constexpr (P1ONLY) {  // no P2 / P3: the next unit's opponent rows right away
+                if (jn < nb) prefetch_opp(jn);
+            } else {
+                prefetch_own(j);
+            }
+        }
         if constexpr (!P1ONLY) {
 
         // ------------------------------------------------------------------------------------------ P2a: card rows
@@ -534,9 +588,11 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
         };
         p3_load(0, gA, aA);
         __syncthreads();  // B2: card rows done, S may be overwritten, the row table may be replaced
+        stamp(it, 2);
         if (tid == 0 && jn < nb) {
             mbar_expect_tx(&bars[2], kRowIdxBytes);
             bulk_g2s(smem + kRowIdxOff, blob_g + (size_t)jn * kBlobBytes + kBlobA, kRowIdxBytes, &bars[2]);
+            if constexpr (kPfPhase) prefetch_opp(jn);
         }
         // card-row sums cs[f][card] and total tf[f] of fold vector f (total = half the sum of its card rows): from the gathered
         // sums csd, or - kLin - as the combination FoldLinFHP of the showdown vectors' row totals
@@ -585,6 +641,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
                 static_for<0, NF>([&](auto F) { fold_finish(F); });
             }
             __syncthreads();  // B3
+            stamp(it, 3);
             const int b0 = 3 * tid;
 #pragma unroll
             for (int v = 0; v < NSD; ++v) {
@@ -598,6 +655,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
             }
         }
         __syncthreads();  // B4: prefix arrays complete
+        stamp(it, 4);
 
         // ------------------------------------------------------------------------------------------ P3: values, bottom-up
         auto p3_hand = [&](int k, const float (&gown)[NOWN], float (&av)[NOWN]) {
@@ -712,6 +770,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
             p1_load(jn, reinterpret_cast<const int16_t*>(smem + kBlobOff + (buf ^ 1) * kBlobA + kRecBytes));
         }
         __syncthreads();  // B5: S / Er / tables of this board are free
+        stamp(it, 5);
     }
     // merge into the device-wide sums (integer adds: exact in any order)
     __syncthreads();
@@ -1195,6 +1254,19 @@ extern "C" int prl_board_avg_flush(const prl_board_game_t* g, int p, int due, in
     prl::count_launch();
     return prl::check(cudaGetLastError(), "prl_board_avg_flush");
 }
+
+#if PRL_BV_STAMPS
+// phase stamps of the last board_sweep_kernel launch (see stamp()): out[kStampCtas][kStampUnits][kStampSlots] int64, then cleared;
+// shape[3] = the three dimensions.  Exported by PRL_BV_STAMPS builds only.
+extern "C" int prl_board_stamps(int64_t* out, int32_t* shape) {
+    shape[0] = kStampCtas;
+    shape[1] = kStampUnits;
+    shape[2] = kStampSlots;
+    if (int e = prl::check(cudaMemcpyFromSymbol(out, g_stamps, sizeof(g_stamps)), "prl_board_stamps: copy")) return e;
+    static const long long zeros[kStampCtas * kStampUnits * kStampSlots] = {};
+    return prl::check(cudaMemcpyToSymbol(g_stamps, zeros, sizeof(g_stamps)), "prl_board_stamps: clear");
+}
+#endif
 
 extern "C" int prl_board_collect(const prl_board_game_t* g, int n_arr, const int16_t* sym_perm, int n_sym, float* out, int ld,
                                  prl_stream_t stream) {

@@ -11,16 +11,20 @@ from pokerrl_b200.csrc import build as B  # noqa: E402
 
 # switches left in csrc/cfr_board.cu: each accepted change against its predecessor (the rejected ones were removed from the
 # source)
-_ON = dict(RED=1, P1PIPE=1, FOLDLIN=1, ERT=1, ROWTOTF=1, NEWTON=1)
+_ON = dict(RED=1, P1PIPE=1, FOLDLIN=1, ERT=1, ROWTOTF=1, NEWTON=1, PF=1, STAMPS=0)
 VARIANTS = {
     "final": dict(_ON),
-    "base": dict(RED=0, P1PIPE=0, FOLDLIN=0, ERT=0, ROWTOTF=0, NEWTON=1),
+    "base": dict(RED=0, P1PIPE=0, FOLDLIN=0, ERT=0, ROWTOTF=0, NEWTON=1, PF=0, STAMPS=0),
     "no_red": dict(_ON, RED=0),
     "no_p1pipe": dict(_ON, P1PIPE=0),
     "no_foldlin": dict(_ON, FOLDLIN=0),
     "no_ert": dict(_ON, ERT=0),
     "no_rowtotf": dict(_ON, ROWTOTF=0),
     "no_newton": dict(_ON, NEWTON=0),
+    "pf0": dict(_ON, PF=0),
+    # phase stamps (tools/board_phases.py) of the kept schedule and of the previous one
+    "stamps": dict(_ON, STAMPS=1),
+    "stamps_pf0": dict(_ON, PF=0, STAMPS=1),
 }
 
 
