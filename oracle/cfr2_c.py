@@ -38,6 +38,8 @@ def lib():
         L.orc2_fill_uniform.argtypes = [tp]
         L.orc2_reach.argtypes = [tp, C.c_void_p]
         L.orc2_values.argtypes = [tp, C.c_void_p, C.c_int, C.c_int]
+        L.orc2_values_levels.argtypes = [tp, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]
+        L.orc2_regret_match.argtypes = [tp]
         L.orc2_exploitability.argtypes = [tp, C.c_void_p]
         L.orc2_regret_update.argtypes = [tp, C.c_int, C.c_int, C.c_int]
         L.orc2_avg_update.argtypes = [tp, C.c_int, C.c_int, C.c_int, C.c_int]
@@ -45,7 +47,8 @@ def lib():
         L.orc2_fold_row.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p]
         L.orc2_showdown_row.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                         C.c_double, C.c_void_p]
-        for f in ("orc2_prepare", "orc2_fill_uniform", "orc2_reach", "orc2_values", "orc2_exploitability",
+        for f in ("orc2_prepare", "orc2_fill_uniform", "orc2_reach", "orc2_values", "orc2_values_levels", "orc2_regret_match",
+                  "orc2_exploitability",
                   "orc2_regret_update", "orc2_avg_update", "orc2_average_strategy", "orc2_fold_row", "orc2_showdown_row"):
             getattr(L, f).restype = None
         _lib = L

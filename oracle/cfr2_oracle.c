@@ -202,10 +202,12 @@ void orc2_reach(orc2_t* t, const double* strat) {
 }
 
 /* ---- bottom-up values (+ best response if with_br) of the seats in mask (ValueFiller.py:21-101); fills ev / ev_br.
- * The reference always evaluates both seats with BR (mask 3, with_br 1); the lean form is what a CFR half-iteration needs. */
-void orc2_values(orc2_t* t, const double* strat, int mask, int with_br) {
+ * The reference always evaluates both seats with BR (mask 3, with_br 1); the lean form is what a CFR half-iteration needs.
+ * orc2_values_levels sweeps levels d_hi .. 0 only and, if keep_chance, leaves the chance nodes' rows as the caller set them:
+ * the trunk of a game whose chance-node rows were summed elsewhere (oracle/cfr2_chunked.py). */
+void orc2_values_levels(orc2_t* t, const double* strat, int mask, int with_br, int d_hi, int keep_chance) {
     const int R = t->R;
-    for (int d = t->n_levels - 1; d >= 0; --d) {
+    for (int d = d_hi; d >= 0; --d) {
         const int lo = (int)t->level_start[d], hi = (int)t->level_start[d + 1];
 #pragma omp parallel for schedule(dynamic, 16)
         for (int n = lo; n < hi; ++n) {
@@ -232,6 +234,7 @@ void orc2_values(orc2_t* t, const double* strat, int mask, int with_br) {
                 continue;
             }
             if (k == K_CHANCE) { /* ValueFiller.py:76-78 with board weights; suit symmetrisation (DESIGN.md) */
+                if (keep_chance) continue;
                 double* w = (double*)malloc(sizeof(double) * (size_t)R * 2);
                 for (int p = 0; p < 2; ++p)
                     for (int br = 0; br < (with_br ? 2 : 1); ++br) {
@@ -276,6 +279,28 @@ void orc2_values(orc2_t* t, const double* strat, int mask, int with_br) {
                     evq[h] = v;
                     if (with_br) brq[h] = b;
                 }
+            }
+        }
+    }
+}
+
+void orc2_values(orc2_t* t, const double* strat, int mask, int with_br) {
+    orc2_values_levels(t, strat, mask, with_br, t->n_levels - 1, 0);
+}
+
+/* strategy = regret matching of the stored regrets at every decision node (CFRPlus.py:43-63) */
+void orc2_regret_match(orc2_t* t) {
+    const int R = t->R;
+#pragma omp parallel for schedule(dynamic, 64)
+    for (int n = 0; n < t->n_nodes; ++n) {
+        if (t->kind[n] > K_P1 || t->n_children[n] == 0) continue;
+        const int A = t->n_children[n], fs = t->slot[t->first_child[n]];
+        for (int h = 0; h < R; ++h) {
+            double s = 0.0;
+            for (int a = 0; a < A; ++a) s += fmax(t->regret[(size_t)(fs + a) * R + h], 0.0);
+            for (int a = 0; a < A; ++a) {
+                const double r = fmax(t->regret[(size_t)(fs + a) * R + h], 0.0);
+                t->strat[(size_t)(fs + a) * R + h] = (s > 0.0) ? r / s : 1.0 / (double)A;
             }
         }
     }
