@@ -28,8 +28,8 @@ typedef void* prl_stream_t; /* cudaStream_t */
 /* bumped whenever a struct below changes; prl_abi_version() returns the value the library was built with
    (2: prl_tree_t gained board_hand_rec / node_rec2 / work_rec2 / level_nfold; 3: board engine, legacy LUT natives;
     4: prl_board_sweep / prl_board_trunk take the algorithm; prl_tree_t gained the all-in terminals of two-card games: level_nallin / allin_nodes / allin_pot / allin_tiles /
-    allin_partial; 5: prl_board_update_cfrp / prl_board_avg_flush) */
-#define PRL_ABI_VERSION 5
+    allin_partial; 5: prl_board_update_cfrp / prl_board_avg_flush; 6: prl_board_policy_query) */
+#define PRL_ABI_VERSION 6
 
 /* node kinds (game/_/tree/_/nodes.py:8-62 + ValueFiller.py:34-62) */
 enum {
@@ -329,6 +329,20 @@ int prl_board_trunk(const prl_board_game_t* g, const prl_trunk_t* t, int eval, i
  * stride per board} in the strength-ordered table and in a natural-order table of stride ld. */
 int prl_board_permute(const prl_board_game_t* g, int rows_per_board, const int64_t* row_src, const int64_t* row_dst,
                       float* sorted_tab, float* natural_tab, int ld, int to_natural, prl_stream_t stream);
+
+/* An agent's answers from its strength-ordered tables (EvalAgentBase.get_a_probs_for_each_hand for the post-deal decision nodes
+ * of n_boards boards, one CTA per board).  The agent: rows = DEVICE float[n_cls][14][ldb] in the board-major row layout of
+ * prl_board_rows, keys = DEVICE int64[n_cls] ascending class keys, pos_hand = DEVICE int16[n_cls][n_live] (the hand ids of the
+ * representative's blob: strength position -> hand).  A key packs the five sorted cards base 64 (holdem_boards.canonical_boards);
+ * iso != 0: the query board's key is the minimum over the 24 suit permutations, the FIRST minimal one in itertools.permutations
+ * order maps its hands onto the representative's; iso == 0: the board's own key.  boards = DEVICE int8[n_boards][5];
+ * out_index = DEVICE int32[n_boards][6]: for the compiled shape's decision nodes in ascending local id, the index d of the node in
+ * out (-1: not wanted); actions = discrete action of local node i in bits 4i..4i+3.  Writes out[d][h][a] (DEVICE float
+ * [.][1326][n_actions], natural hand order): the row of the child with action a at hand h's position, 0 for blocked hands and
+ * for actions the node does not allow.  A board whose key the agent does not hold sets *miss (DEVICE int32) to 1. */
+int prl_board_policy_query(const float* rows, const int64_t* keys, const int16_t* pos_hand, int n_cls, int iso,
+                           const int8_t* boards, int n_boards, const int32_t* out_index, uint64_t actions, int n_actions,
+                           float* out, int32_t* miss, prl_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * 7-card Hold'em hand evaluation (replaces lib_hand_eval.so; int32 strength, higher = better, identical encoding incl.

@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("PRL_LIB_PATH") or os.path.join(_HERE, "lib", "libpoke
 # enums of include/pokerrl_b200.h
 KIND_P0, KIND_P1, KIND_CHANCE, KIND_FOLD, KIND_SHOWDOWN, KIND_SHOWDOWN_ALLIN = range(6)
 ALGO_VANILLA, ALGO_CFR_PLUS, ALGO_LINEAR = 0, 1, 2
-ABI_VERSION = 5  # include/pokerrl_b200.h: PRL_ABI_VERSION
+ABI_VERSION = 6  # include/pokerrl_b200.h: PRL_ABI_VERSION
 STRAT_F32, STRAT_UNIFORM64, STRAT_AVG_F64, STRAT_AVG_SUM, STRAT_AVG_F32 = range(5)
 
 
@@ -151,8 +151,10 @@ def lib():
     L.prl_board_trunk.argtypes = [gp, C.POINTER(PrlTrunk), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                   C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_void_p]
     L.prl_board_trunk.restype = C.c_int
+    L.prl_board_policy_query.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                         C.c_uint64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     for f in ("prl_board_layout", "prl_board_grid", "prl_board_shape_ok", "prl_board_build_tables", "prl_board_sweep",
-              "prl_board_update_cfrp", "prl_board_avg_flush", "prl_board_collect", "prl_board_permute"):
+              "prl_board_update_cfrp", "prl_board_avg_flush", "prl_board_collect", "prl_board_permute", "prl_board_policy_query"):
         getattr(L, f).restype = C.c_int
     ep = C.POINTER(PrlEnvCfg)
     L.prl_env_state_fields.restype = C.c_int

@@ -65,7 +65,112 @@ def _fill_shape(g, st):
         g.n_children[i], g.acted_last[i], g.pot[i] = st["n_children"][i], st["acted_last"][i], st["pot"][i]
 
 
-class BoardCFRSolver:
+def board_mask(boards):
+    mask = np.zeros(boards.shape[0], np.uint64)
+    for k in range(boards.shape[1]):
+        mask |= (np.uint64(1) << boards[:, k].astype(np.uint64))
+    return mask
+
+
+def build_board_blobs(rules, boards, t_blob, dev):
+    """per-board tables of `boards` (int8 [n, 5]) into t_blob[:n]: hand ranks (prl_hand_rank_boards), then
+    prl_board_build_tables, 16 384 boards per launch"""
+    from pokerrl_b200.hand_eval import hand_rank_all_hands_on_given_boards
+    boards = np.ascontiguousarray(boards, np.int8)
+    nb = boards.shape[0]
+    lut = rules.get_lut_holder()
+    t_hc = torch.from_numpy(np.ascontiguousarray(lut.LUT_IDX_2_HOLE_CARDS, np.int8)).to(dev)
+    t_mask = torch.from_numpy(board_mask(boards).view(np.int64)).to(dev)
+    CH = 16384
+    for i in range(0, nb, CH):
+        n = min(CH, nb - i)
+        ranks = hand_rank_all_hands_on_given_boards(boards[i:i + n], device=dev)
+        nat.call("prl_board_build_tables", C.c_void_p(ranks.data_ptr()), C.c_void_p(t_mask[i:i + n].data_ptr()),
+                 C.c_void_p(t_hc.data_ptr()), n, C.c_void_p(t_blob[i:i + n].data_ptr()), _stream(dev))
+
+
+def board_game(st, rules, n_boards, ld, n_sym, grid=0):
+    """prl_board_game_t of a post-deal subtree `st` over n_boards boards, without buffers: shape, eq_const, the fixed-point
+    format of the chance sums (which depends on n_sym, not on the boards) and the board-major row layout.
+    Returns (g, rows_per_board, local_rows = {local child node: (row on board 0, stride per board)})."""
+    g = nat.PrlBoardGame()
+    _fill_shape(g, st)
+    g.n_boards, g.n_range, g.ld, g.n_deck = n_boards, rules.RANGE_SIZE, ld, rules.N_CARDS_IN_DECK
+    n_hole = rules.N_HOLE_CARDS
+    g.eq_const = math.comb(g.n_deck, n_hole) / math.comb(g.n_deck - n_hole, n_hole)
+    # fixed point: |sum| <= n_sym * K * max pot / 2 with headroom; 62 value bits
+    bound = max(n_sym, 1) * g.eq_const * max(st["pot"]) * 0.5 * 4.0
+    g.frac_bits = 62 - int(math.ceil(math.log2(bound)))
+    n_local = st["n_local"]
+    dec = [i for i in range(n_local) if st["kind"][i] <= 1]
+    rows_per_board = sum(st["n_children"][i] for i in dec)
+    # board-major rows: everything a (board, seat) unit touches is contiguous - row(i, j) = j * rows_per_board + row_of[i]
+    row_of, rpb = (C.c_int32 * 16)(), C.c_int32(0)
+    nat.call("prl_board_rows", row_of, C.byref(rpb))
+    assert rpb.value == rows_per_board
+    local_rows = {}  # local child node -> (row on board 0, stride per board)
+    for i in range(n_local):
+        g.row0[i], g.row_m[i] = -1, 0
+    for d in dec:
+        for a in range(st["n_children"][d]):
+            c = st["first_child"][d] + a
+            g.row0[c], g.row_m[c] = row_of[c], rpb.value
+            local_rows[c] = (int(row_of[c]), rpb.value)
+    g.grid = int(grid) if grid else int(nat.lib().prl_board_grid())
+    return g, rows_per_board, local_rows
+
+
+class _BoardTrunk:
+    """The pre-deal trunk shared by the solver and the policy evaluator: a one-board flat tree carries the trunk and the
+    shape of the post-deal subtree; the trunk is swept by prl_board_trunk / the level kernels over its own small buffers."""
+
+    def _init_trunk(self, game_cls, env_args, dev):
+        self.ft1 = FlatTree(game_cls, env_args, board_spec=_one_board_spec())
+        st = self.ft1.board_subtree()
+        if st is None:
+            raise ValueError("the game does not have ONE chance layer with a <= 16-node post-deal subtree")
+        self.st = st
+        self.chance_level = st["chance_level"]
+        self.chance_node = st["chance_node"]
+        self.R = game_cls.RULES.RANGE_SIZE
+        # trunk: level sweeps over levels 0 .. chance_level of the one-board tree; the symmetrisation over the suit
+        # permutations happens in prl_board_collect / prl_board_trunk (integer sums), not in the level kernels
+        self.trunk = DeviceTree(self.ft1, dev)
+        self.trunk.desc.n_sym = 0
+        self.trunk.desc.sym_perm = None
+        self.bufs = TreeBuffers(self.trunk)
+        self.ld = self.trunk.ld
+
+    def _trunk_desc(self, bufs, modes):
+        ft, t = self.ft1, nat.PrlTrunk()
+        n = self.chance_node + 1
+        assert n <= 8 and int(ft.level_start[self.chance_level + 1]) == n, "the trunk must be the first nodes of the flat tree"
+        t.n_nodes, t.chance_node, t.n_buf_nodes, t.ld, t.n_range = n, self.chance_node, self.trunk.n_nodes, self.ld, self.R
+        t.mode[0], t.mode[1] = modes
+        t.eq_const = self.g.eq_const
+        for i in range(n):
+            t.kind[i], t.first_child[i], t.n_children[i] = int(ft.kind[i]), int(ft.first_child[i]), int(ft.n_children[i])
+            t.acted_last[i], t.pot[i] = int(ft.acted_last[i]), float(ft.pot[i])
+            t.first_slot[i] = int(ft.first_slot[i]) if ft.first_slot[i] >= 0 else 0
+        t.hand_cards = self.trunk.t_hand_cards.data_ptr()
+        t.reach, t.ev, t.ev_br = bufs.reach.data_ptr(), bufs.ev.data_ptr(), bufs.ev_br.data_ptr()
+        t.regret, t.strat, t.avg = bufs.regret.data_ptr(), bufs.strat.data_ptr(), bufs.avg.data_ptr()
+        return t
+
+    def _trunk_reach_row(self, bufs, seat):
+        return C.c_void_p(bufs.reach.data_ptr() + 4 * (seat * self.trunk.n_nodes + self.chance_node) * self.ld)
+
+    def _reach_trunk(self, bufs, mask, algo, upd_p, modes):
+        nat.call("prl_reach_levels", C.byref(self.trunk.desc), C.byref(bufs.desc), mask, algo, upd_p, self.iter_counter,
+                 self.delay, nat.modes(*modes), 0, self.chance_level, _stream(self.device))
+
+    @property
+    def n_trunk_slots(self):
+        """table rows of the trunk: the first slots of every flat tree of the game (its children come before the deal)"""
+        return self.ft1.n_slots - sum(self.st["n_children"][i] for i in range(self.st["n_local"]) if self.st["kind"][i] <= 1)
+
+
+class BoardCFRSolver(_BoardTrunk):
     def __init__(self, game_cls, env_args, board_spec=None, algo="CFRPlus", delay=0, device=None, rank=0, world=1,
                  group=None, grid=0, reduce_fn=None):
         if algo not in ALGOS:
@@ -97,77 +202,30 @@ class BoardCFRSolver:
     # ------------------------------------------------------------------------------------------------ construction
     def _build(self, rules, spec, grid):
         dev, L = self.device, self.L
-        # structure: a one-board flat tree carries the trunk and the shape of the post-deal subtree
-        self.ft1 = FlatTree(self.game_cls, self.env_args, board_spec=_one_board_spec())
-        st = self.ft1.board_subtree()
-        if st is None:
-            raise ValueError("the game does not have ONE chance layer with a <= 16-node post-deal subtree")
-        self.st = st
-        self.chance_level = st["chance_level"]
-        self.chance_node = st["chance_node"]
+        self._init_trunk(self.game_cls, self.env_args, dev)
+        st = self.st
         sel = np.arange(self.rank, spec.boards.shape[0], self.world)
         self.board_ids = sel
         self.boards = np.ascontiguousarray(spec.boards[sel], np.int8)
         nb = self.n_boards = int(sel.size)
         self.n_boards_total = int(spec.boards.shape[0])
-        self.R = rules.RANGE_SIZE
-        # trunk: level sweeps over levels 0 .. chance_level of the one-board tree; the symmetrisation over the suit
-        # permutations happens in prl_board_collect (integer sums), not in the level kernels
-        self.trunk = DeviceTree(self.ft1, dev)
-        self.trunk.desc.n_sym = 0
-        self.trunk.desc.sym_perm = None
-        self.bufs = TreeBuffers(self.trunk)
         self.ops = TreeOps(self.trunk, self.bufs)
         self._eval_bufs = None
-        self.ld = self.trunk.ld
         sp = spec.sym_perm
         self.t_sym = None if sp is None else torch.from_numpy(np.ascontiguousarray(sp, np.int16)).to(dev)
         self.n_sym = 0 if sp is None else int(sp.shape[0])
         # per-board tables
-        from pokerrl_b200.hand_eval import hand_rank_all_hands_on_given_boards
         self.t_blob = torch.empty((max(nb, 1), L["blob"]), dtype=torch.uint8, device=dev)
-        lut = rules.get_lut_holder()
-        t_hc = torch.from_numpy(np.ascontiguousarray(lut.LUT_IDX_2_HOLE_CARDS, np.int8)).to(dev)
-        mask = np.zeros(nb, np.uint64)
-        for k in range(self.boards.shape[1]):
-            mask |= (np.uint64(1) << self.boards[:, k].astype(np.uint64))
-        t_mask = torch.from_numpy(mask.view(np.int64)).to(dev)
-        CH = 16384
-        for i in range(0, nb, CH):
-            n = min(CH, nb - i)
-            ranks = hand_rank_all_hands_on_given_boards(self.boards[i:i + n], device=dev)
-            nat.call("prl_board_build_tables", C.c_void_p(ranks.data_ptr()), C.c_void_p(t_mask[i:i + n].data_ptr()),
-                     C.c_void_p(t_hc.data_ptr()), n, C.c_void_p(self.t_blob[i:i + n].data_ptr()), _stream(dev))
+        build_board_blobs(rules, self.boards, self.t_blob, dev)
         torch.cuda.synchronize(dev)
         self.t_prob = torch.from_numpy(np.ascontiguousarray(spec.board_prob[sel], np.float32)).to(dev)
         self.t_mult = torch.from_numpy(np.ascontiguousarray(spec.board_mult[sel], np.float32)).to(dev)
         n_local = st["n_local"]
         dec = [i for i in range(n_local) if st["kind"][i] <= 1]
-        self.rows_per_board = sum(st["n_children"][i] for i in dec)
+        g, self.rows_per_board, self.local_rows = board_game(st, rules, nb, self.ld, self.n_sym, grid)
         self.n_rows = nb * self.rows_per_board
         self.regret = torch.zeros((max(self.n_rows, 1), L["ldb"]), dtype=torch.float32, device=dev)
         self.avg = torch.zeros_like(self.regret)
-        g = nat.PrlBoardGame()
-        _fill_shape(g, st)
-        g.n_boards, g.n_range, g.ld, g.n_deck = nb, self.R, self.ld, rules.N_CARDS_IN_DECK
-        n_hole = rules.N_HOLE_CARDS
-        g.eq_const = math.comb(g.n_deck, n_hole) / math.comb(g.n_deck - n_hole, n_hole)
-        # fixed point: |sum| <= n_sym * K * max pot / 2 with headroom; 62 value bits
-        bound = max(self.n_sym, 1) * g.eq_const * max(st["pot"]) * 0.5 * 4.0
-        g.frac_bits = 62 - int(math.ceil(math.log2(bound)))
-        # board-major rows: everything a (board, seat) unit touches is contiguous - row(i, j) = j * rows_per_board + row_of[i]
-        row_of, rpb = (C.c_int32 * 16)(), C.c_int32(0)
-        nat.call("prl_board_rows", row_of, C.byref(rpb))
-        assert rpb.value == self.rows_per_board
-        self.local_rows = {}  # local child node -> (row on board 0, stride per board)
-        for i in range(n_local):
-            g.row0[i], g.row_m[i] = -1, 0
-        for d in dec:
-            for a in range(st["n_children"][d]):
-                c = st["first_child"][d] + a
-                g.row0[c], g.row_m[c] = row_of[c], rpb.value
-                self.local_rows[c] = (int(row_of[c]), rpb.value)
-        g.grid = int(grid) if grid else int(nat.lib().prl_board_grid())
         g.tables, g.board_prob, g.board_mult = self.t_blob.data_ptr(), self.t_prob.data_ptr(), self.t_mult.data_ptr()
         g.regret, g.avg = self.regret.data_ptr(), self.avg.data_ptr()
         self.w_private = torch.zeros((g.grid, 2, self.R), dtype=torch.int64, device=dev)
@@ -205,22 +263,6 @@ class BoardCFRSolver:
                           + self.n_boards_total * len(dec))
 
     # ------------------------------------------------------------------------------------------------ helpers
-    def _trunk_desc(self, bufs, modes):
-        ft, t = self.ft1, nat.PrlTrunk()
-        n = self.chance_node + 1
-        assert n <= 8 and int(ft.level_start[self.chance_level + 1]) == n, "the trunk must be the first nodes of the flat tree"
-        t.n_nodes, t.chance_node, t.n_buf_nodes, t.ld, t.n_range = n, self.chance_node, self.trunk.n_nodes, self.ld, self.R
-        t.mode[0], t.mode[1] = modes
-        t.eq_const = self.g.eq_const
-        for i in range(n):
-            t.kind[i], t.first_child[i], t.n_children[i] = int(ft.kind[i]), int(ft.first_child[i]), int(ft.n_children[i])
-            t.acted_last[i], t.pot[i] = int(ft.acted_last[i]), float(ft.pot[i])
-            t.first_slot[i] = int(ft.first_slot[i]) if ft.first_slot[i] >= 0 else 0
-        t.hand_cards = self.trunk.t_hand_cards.data_ptr()
-        t.reach, t.ev, t.ev_br = bufs.reach.data_ptr(), bufs.ev.data_ptr(), bufs.ev_br.data_ptr()
-        t.regret, t.strat, t.avg = bufs.regret.data_ptr(), bufs.strat.data_ptr(), bufs.avg.data_ptr()
-        return t
-
     def _trunk(self, bufs, modes, evaluate, p):
         peers, n_peers, off = None, 0, 0
         if self._symm is not None:
@@ -249,16 +291,9 @@ class BoardCFRSolver:
             dist.all_reduce(view, op=dist.ReduceOp.SUM, group=self.group)
         self.n_allreduce += 1
 
-    def _trunk_reach_row(self, bufs, seat):
-        return C.c_void_p(bufs.reach.data_ptr() + 4 * (seat * self.trunk.n_nodes + self.chance_node) * self.ld)
-
     def _levels(self, bufs, mask, with_br, algo, upd_p, modes, hi, lo, phase):
         nat.call("prl_value_levels", C.byref(self.trunk.desc), C.byref(bufs.desc), mask, int(with_br), algo, upd_p,
                  self.iter_counter, self.delay, nat.modes(*modes), hi, lo, phase, _stream(self.device))
-
-    def _reach_trunk(self, bufs, mask, algo, upd_p, modes):
-        nat.call("prl_reach_levels", C.byref(self.trunk.desc), C.byref(bufs.desc), mask, algo, upd_p, self.iter_counter,
-                 self.delay, nat.modes(*modes), 0, self.chance_level, _stream(self.device))
 
     def _sweep_begin(self, bufs, p, evaluate, src_own, src_opp):
         if not evaluate and self.algo == nat.ALGO_CFR_PLUS:
@@ -480,3 +515,337 @@ class BoardCFRSolver:
         self.bufs.avg.copy_(state["trunk_avg"])
         with torch.cuda.device(self.device):
             self._reach_trunk(self.bufs, 3, -1, -1, self.modes)
+
+
+# ==================================================================================================================== policy evaluation
+def board_keys(boards):
+    """int64 key of each board: its sorted cards packed base 64 (holdem_boards.canonical_boards)"""
+    b = np.sort(np.asarray(boards, np.int64), axis=1)
+    key = np.zeros(b.shape[0], np.int64)
+    for i in range(b.shape[1]):
+        key = key * 64 + b[:, i]
+    return key
+
+
+def _decision_locals(st):
+    """post-deal decision nodes, ascending local id (the columns of prl_board_policy_query's out_index)"""
+    return [i for i in range(st["n_local"]) if st["kind"][i] <= 1 and st["n_children"][i] > 0]
+
+
+def chunk_row_map(ft, st, local_rows):
+    """(src, dst): for every row of the post-deal decision nodes, {row on board 0, stride per board} in the strength-ordered
+    table and in the slot table of the flat tree `ft` over a chunk of boards (the prl_board_permute descriptors)"""
+    src, dst = [], []
+    for i, (r0, m) in sorted(local_rows.items()):
+        src += [r0, m]
+        dst += [int(ft.slot[st["node_base"][i] + st["node_k"][i]]), st["node_m"][i]]
+    return src, dst
+
+
+def abstract_fingerprint(ft):
+    """identity of the betting structure of a flat tree (any board spec): kinds, actions, pots and fan-outs of its abstract
+    nodes - equal for every spec of one game and stack"""
+    import hashlib
+    a = np.array([(n.kind, n.action, n.pot, len(n.children), n.parent, n.acted_last) for n in ft.abs_nodes], np.int64)
+    return hashlib.sha1(a.tobytes()).hexdigest()
+
+
+class BoardPolicyEvaluator(_BoardTrunk):
+    """Exploitability of an agent's strategy on a game the board engine supports (single GPU), with the strategy supplied
+    chunk by chunk over the boards of a BoardSpec, so that it never has to exist for the whole game at once.
+
+    Spec: default = the game's suit-isomorphism classes, the semantics of PublicTree (the agent is queried on the
+    representatives, which is exact for suit-symmetric agents); BoardSpec.full_game(rules, isomorphic=False) = every deal
+    (2 598 960 boards in Flop5Holdem), exact for any agent.
+
+    Per chunk of boards: a structure-only PublicTree over the chunk's slice of the spec is filled from the agent
+    (PublicTree.agent_strategy_table: one batched get_a_probs_for_public_tree, or one get_a_probs_for_each_hand call per decision
+    node - about 807 k calls over the 134 459 classes, slow but supported; float64 answers are rounded to float32), the boards'
+    tables are built (build_board_blobs), the post-deal rows are moved into each board's strength order (prl_board_permute) and
+    the evaluation sweep of each seat runs on them as they are (prl_board_sweep, src 1).  Its fixed-point chance sums are added
+    into an int64 accumulator: integer addition makes the result independent of the chunking.  The trunk's rows come from the
+    first chunk's answers (mode STRAT_AVG_F32) and its reach pass runs before the first sweep, which reads the opponent's reach
+    at the chance node.  After the last chunk one prl_board_trunk evaluation gives the exploitability of each seat.
+
+    Device memory is chunk-sized, allocated once:  chunk * bytes_per_board  with
+        bytes_per_board = blob (15 392) + strength-ordered rows (rows_per_board * 1088 * 4)
+                          + slot-table rows (rows_per_board * ld * 4) + the batched answers (n_dec * 1326 * N_ACTIONS * 4)
+                          + hand ranks (1326 * 4)
+    (Flop5Holdem: 14 rows, ld 1328, 6 decision nodes, 3 actions: 245 KB per board), plus the trunk and the chance sums.
+    Default chunk = min(65 536, n_boards, free device memory / 2 / bytes_per_board)."""
+
+    MAX_CHUNK = 65536
+
+    def __init__(self, env_bldr, stack_size=None, board_spec=None, chunk=None, device=None):
+        self.device = dev = _require_cuda(device)
+        self.env_bldr, self.stack_size = env_bldr, stack_size
+        game_cls = env_bldr.env_cls
+        self.env_args = env_bldr.args_for_stack(stack_size)
+        rules = self.rules = game_cls.RULES
+        self.spec = board_spec if board_spec is not None else BoardSpec.full_game(rules)
+        self.iter_counter, self.delay = 0, 0
+        self.ev_normalizer = game_cls.EV_NORMALIZER
+        L = self.L = board_layout()
+        n_actions = env_bldr.N_ACTIONS
+        with torch.cuda.device(dev):
+            self._init_trunk(game_cls, self.env_args, dev)
+            st = self.st
+            sp = self.spec.sym_perm
+            self.n_sym = 0 if sp is None else int(sp.shape[0])
+            self.t_sym = None if sp is None else torch.from_numpy(np.ascontiguousarray(sp, np.int16)).to(dev)
+            self.n_boards_total = nb = int(self.spec.boards.shape[0])
+            g, rpb, self.local_rows = board_game(st, rules, 0, self.ld, self.n_sym)
+            self.rows_per_board = rpb
+            n_dec = len(_decision_locals(st))
+            self.bytes_per_board = (L["blob"] + rpb * L["ldb"] * 4 + rpb * self.ld * 4 + n_dec * self.R * n_actions * 4
+                                    + self.R * 4)
+            if chunk is None:
+                free, _ = torch.cuda.mem_get_info(dev)
+                chunk = min(self.MAX_CHUNK, free // 2 // self.bytes_per_board)
+            self.chunk = max(1, min(int(chunk), nb))
+            n = self.chunk
+            self.t_blob = torch.empty((n, L["blob"]), dtype=torch.uint8, device=dev)
+            self.rows = torch.zeros((n * rpb, L["ldb"]), dtype=torch.float32, device=dev)
+            self.nat_tab = torch.zeros((self.n_trunk_slots + n * rpb, self.ld), dtype=torch.float32, device=dev)
+            self.t_prob = torch.zeros(n, dtype=torch.float32, device=dev)
+            self.t_mult = torch.zeros(n, dtype=torch.float32, device=dev)
+            self.w_private = torch.zeros((g.grid, 2, self.R), dtype=torch.int64, device=dev)
+            self.w_total = torch.zeros((4, self.R), dtype=torch.int64, device=dev)
+            self.w_acc = torch.zeros_like(self.w_total)
+            self._expl = torch.zeros(2, dtype=torch.float32, device=dev)
+            g.tables, g.board_prob, g.board_mult = self.t_blob.data_ptr(), self.t_prob.data_ptr(), self.t_mult.data_ptr()
+            # evaluation with src 1 reads the strategy rows as they are and never the regrets: one table serves both
+            g.regret = g.avg = self.rows.data_ptr()
+            g.w_private, g.w_total = self.w_private.data_ptr(), self.w_total.data_ptr()
+            self.g = g
+        self.n_nodes = int(self.ft1.level_start[self.chance_level + 1]) + nb * st["n_local"]
+        self.n_nonterm = (int((self.ft1.kind[:self.chance_node + 1] <= nat.KIND_CHANCE).sum())
+                          + nb * len([i for i in range(st["n_local"]) if st["kind"][i] <= 1]))
+        self.times = {}
+
+    def _chunk_tree(self, lo, hi):
+        from pokerrl_b200.game.PublicTree import PublicTree
+        s = self.spec
+        spec = BoardSpec(s.boards[lo:hi], s.board_prob[lo:hi], s.board_mult[lo:hi], s.sym_perm,
+                         "boards %d .. %d of: %s" % (lo, hi, s.note))
+        pt = PublicTree(self.env_bldr, self.stack_size, stop_at_street=None, put_out_new_round_after_limit=True,
+                        device=self.device, board_spec=spec)
+        pt.build_structure()
+        return pt
+
+    def evaluate(self, agent, profile=False):
+        """exploitability of each seat in chips, numpy float64 [2] (the analogue of PublicTree's root.exploitability).
+        profile=True synchronises between the phases and leaves their wall times (s) in self.times."""
+        import time
+        dev, g, R = self.device, self.g, self.R
+        times = {"agent query": 0.0, "table build": 0.0, "sweeps": 0.0}
+        modes = [nat.STRAT_AVG_F32, nat.STRAT_AVG_F32]
+
+        def tick(key, t0):
+            if profile:
+                torch.cuda.synchronize(dev)
+                t1 = time.perf_counter()
+                times[key] += t1 - t0
+                return t1
+            return t0
+
+        with torch.cuda.device(dev):
+            self.w_acc.zero_()
+            nts = self.n_trunk_slots
+            for lo in range(0, self.n_boards_total, self.chunk):
+                hi = min(lo + self.chunk, self.n_boards_total)
+                n = hi - lo
+                t0 = time.perf_counter()
+                pt = self._chunk_tree(lo, hi)
+                ft = pt.flat
+                tab = self.nat_tab[:ft.n_slots]
+                got = pt.agent_strategy_table(agent, out=tab)
+                if not isinstance(got, torch.Tensor):  # answered node by node on the host
+                    tab[:, :R].copy_(torch.from_numpy(np.ascontiguousarray(got, np.float32)))
+                t0 = tick("agent query", t0)
+                build_board_blobs(self.rules, self.spec.boards[lo:hi], self.t_blob, dev)
+                self.t_prob[:n].copy_(torch.from_numpy(np.ascontiguousarray(self.spec.board_prob[lo:hi], np.float32)))
+                self.t_mult[:n].copy_(torch.from_numpy(np.ascontiguousarray(self.spec.board_mult[lo:hi], np.float32)))
+                g.n_boards = n
+                src, dst = chunk_row_map(ft, pt.flat.board_subtree(), self.local_rows)
+                t_src = torch.tensor(src, dtype=torch.int64, device=dev)
+                t_dst = torch.tensor(dst, dtype=torch.int64, device=dev)
+                nat.call("prl_board_permute", C.byref(g), len(self.local_rows), C.c_void_p(t_src.data_ptr()),
+                         C.c_void_p(t_dst.data_ptr()), C.c_void_p(self.rows.data_ptr()), C.c_void_p(tab.data_ptr()), self.ld, 0,
+                         _stream(dev))
+                if lo == 0:  # the trunk's rows, then its reach: the sweeps read the opponent's reach at the chance node
+                    self.bufs.avg[:nts].copy_(tab[:nts])
+                    self._reach_trunk(self.bufs, 3, -1, -1, modes)
+                t0 = tick("table build", t0)
+                for p in (0, 1):  # prl_board_sweep zeroes the arrays it writes at every launch: accumulate outside
+                    nat.call("prl_board_sweep", C.byref(g), p, 1, SRC_AVG, SRC_AVG, self._trunk_reach_row(self.bufs, 1 - p), 0, 0,
+                             nat.ALGO_CFR_PLUS, 0.0, 0, _stream(dev))
+                    self.w_acc[2 * p:2 * p + 2] += self.w_total[2 * p:2 * p + 2]
+                tick("sweeps", t0)
+                del pt
+            t0 = time.perf_counter()
+            self.w_total.copy_(self.w_acc)
+            nat.call("prl_board_trunk", C.byref(g), C.byref(self._trunk_desc(self.bufs, modes)), 1, -1, self.n_sym,
+                     C.c_void_p(self.t_sym.data_ptr()) if self.n_sym else None, 0, 0, C.c_void_p(self._expl.data_ptr()), None, 0, 0,
+                     None, nat.ALGO_CFR_PLUS, _stream(dev))
+            e = self._expl.cpu().numpy().astype(np.float64)
+            tick("sweeps", t0)
+        self.times = times
+        return e
+
+
+class BoardPolicyTables:
+    """A board-engine strategy as an agent's own tables, independent of the solver that computed it:
+      rows      float32 [n_cls * rows_per_board, 1088]  strength-ordered post-deal rows (the solver's board-major layout)
+      keys      int64   [n_cls]                          ascending class keys (board_keys of the representatives)
+      pos_hand  int16   [n_cls, 1081]                    strength position -> hand, cut from the boards' tables
+      trunk     float32 [n_trunk_slots, ld]              trunk rows, natural hand order
+    iso: the spec holds suit-isomorphism classes (queries are canonicalised), else raw boards.  Answers for the decision nodes
+    of any flat tree of the game (any board spec, either engine) through prl_board_policy_query."""
+
+    def __init__(self, rows, keys, pos_hand, trunk, iso, actions, fingerprint, spec_id):
+        self.rows, self.keys, self.pos_hand, self.trunk = rows, keys, pos_hand, trunk
+        self.iso, self.actions, self.fingerprint, self.spec_id = bool(iso), int(actions), fingerprint, spec_id
+        self.n_cls = int(keys.shape[0])
+
+    @classmethod
+    def from_solver(cls, s):
+        """the average strategy of a single-GPU BoardCFRSolver: CFR+ after iteration delay + 1 the average rows as they are, at
+        delay + 1 regret matching of the regret rows (CFRPlus.py:83-84); Vanilla / Linear CFR the normalised reach-weighted sums
+        with the uniform fallback (LinearCFR.py:64-71)"""
+        import hashlib
+        if s.world != 1:
+            raise ValueError("a sharded solver holds only its rank's boards")
+        s.flush_average()
+        cfrp = s.algo == nat.ALGO_CFR_PLUS
+        if cfrp and s.iter_counter <= s.delay:
+            raise RuntimeError("CFR+ has no average strategy before iteration delay+1")
+        nb, rpb, st = s.n_boards, s.rows_per_board, s.st
+        groups = [[s.local_rows[c][0] for c in range(st["first_child"][d], st["first_child"][d] + st["n_children"][d])]
+                  for d in _decision_locals(st)]
+        with torch.cuda.device(s.device):
+            if cfrp and s.iter_counter > s.delay + 1:
+                rows = s.avg.clone()
+            else:
+                matching = cfrp  # regret matching at delay + 1, else normalised sums
+                rows = torch.empty_like(s.avg)
+                src = (s.regret if matching else s.avg).view(nb, rpb, -1)
+                dst = rows.view(nb, rpb, -1)
+                for lo in range(0, nb, 8192):
+                    hi = min(lo + 8192, nb)
+                    for idx in groups:
+                        x = src[lo:hi, idx]
+                        if matching:
+                            x = x.clamp(min=0)
+                        tot = x.sum(dim=1, keepdim=True)
+                        ok = (tot > 0) if matching else (tot != 0)
+                        dst[lo:hi, idx] = torch.where(ok, x / torch.where(ok, tot, torch.ones_like(tot)),
+                                                      torch.full_like(x, 1.0 / len(idx)))
+            nts, ft = s.n_trunk_slots, s.ft1
+            if cfrp:
+                trunk = (s.bufs.strat if s.iter_counter == s.delay + 1 else s.bufs.avg)[:nts].clone()
+            else:
+                a = s.bufs.avg[:nts]
+                trunk = torch.zeros_like(a)
+                for n in range(s.chance_node + 1):
+                    if ft.kind[n] <= 1 and ft.first_child[n] >= 0:
+                        fs, A = int(ft.first_slot[n]), int(ft.n_children[n])
+                        tot = a[fs:fs + A].sum(dim=0, keepdim=True)
+                        trunk[fs:fs + A] = torch.where(tot == 0, torch.full_like(a[fs:fs + A], 1.0 / A),
+                                                       a[fs:fs + A] / torch.where(tot == 0, torch.ones_like(tot), tot))
+            L = s.L
+            pos_hand = s.t_blob[:nb, L["sh_off"]:L["sh_off"] + 2 * L["n_live"]].contiguous().view(torch.int16)
+            keys = board_keys(s.boards)
+            if np.any(np.diff(keys) <= 0):  # a spec in another order: rows by ascending key
+                perm = np.argsort(keys, kind="stable")
+                t_perm = torch.from_numpy(perm).to(s.device)
+                rows = rows.view(nb, rpb, -1)[t_perm].reshape(nb * rpb, -1)
+                pos_hand = pos_hand[t_perm]
+                keys = keys[perm]
+            t_keys = torch.from_numpy(keys).to(s.device)
+        spec_id = (int(nb), s.n_sym > 0, hashlib.sha1(keys.tobytes()).hexdigest())
+        return cls(rows, t_keys, pos_hand, trunk, s.n_sym > 0, _packed_actions(s.ft1, st), abstract_fingerprint(s.ft1),
+                   spec_id)
+
+    # ---- queries
+    def _check(self, ft):
+        if abstract_fingerprint(ft) != self.fingerprint:
+            raise ValueError("this agent's tables were computed on a different betting tree (game / stack / bet set)")
+
+    def _query(self, boards, out_index, out, n_actions):
+        dev = out.device
+        miss = torch.zeros(1, dtype=torch.int32, device=dev)
+        t_b = torch.from_numpy(np.ascontiguousarray(boards, np.int8)).to(dev)
+        t_i = torch.from_numpy(np.ascontiguousarray(out_index, np.int32)).to(dev)
+        with torch.cuda.device(dev):
+            nat.call("prl_board_policy_query", C.c_void_p(self.rows.data_ptr()), C.c_void_p(self.keys.data_ptr()),
+                     C.c_void_p(self.pos_hand.data_ptr()), self.n_cls, int(self.iso), C.c_void_p(t_b.data_ptr()), int(t_b.shape[0]),
+                     C.c_void_p(t_i.data_ptr()), self.actions, n_actions, C.c_void_p(out.data_ptr()), C.c_void_p(miss.data_ptr()),
+                     _stream(dev))
+        if int(miss.item()):
+            raise ValueError("a queried board is not in this agent's board spec (%s)"
+                             % ("suit classes" if self.iso else "boards without isomorphism"))
+
+    def answer_tree(self, ft, n_actions):
+        """float32 [n_decision, R, n_actions] on the tables' device for every decision node of `ft` in flat order"""
+        self._check(ft)
+        dev = self.rows.device
+        dec = np.nonzero((ft.kind <= nat.KIND_P1) & (ft.first_child >= 0))[0]
+        dec_idx = np.full(ft.n_nodes, -1, np.int64)
+        dec_idx[dec] = np.arange(dec.size)
+        out = torch.empty((dec.size, ft.R, n_actions), dtype=torch.float32, device=dev)
+        for n in dec[ft.cdepth[dec] == 0]:
+            self._trunk_node(ft, n, out[dec_idx[n]])
+        st = ft.board_subtree()
+        nb = int(st["n_boards_local"])
+        J = np.arange(nb, dtype=np.int64)
+        locs = _decision_locals(st)
+        idx = np.full((nb, len(locs)), -1, np.int64)
+        for d, i in enumerate(locs):
+            idx[:, d] = dec_idx[st["node_base"][i] + J * st["node_m"][i] + st["node_k"][i]]
+        self._query(ft.board_spec.boards, idx, out, n_actions)
+        return out
+
+    def answer_node(self, ft, n, n_actions):
+        """numpy float32 [R, n_actions] at decision node n of `ft` (the one-node form of answer_tree)"""
+        self._check(ft)
+        out = torch.empty((1, ft.R, n_actions), dtype=torch.float32, device=self.rows.device)
+        if ft.cdepth[n] == 0:
+            self._trunk_node(ft, n, out[0])
+            return out[0].cpu().numpy()
+        st = ft.board_subtree()
+        j = int(ft.board[n]) - int(st["first_board"])
+        locs = _decision_locals(st)
+        idx = np.full((1, len(locs)), -1, np.int64)
+        for d, i in enumerate(locs):
+            if st["node_base"][i] + j * st["node_m"][i] + st["node_k"][i] == n:
+                idx[0, d] = 0
+        assert (idx == 0).sum() == 1, "not a post-deal decision node"
+        self._query(ft.board_spec.boards[j:j + 1], idx, out, n_actions)
+        return out[0].cpu().numpy()
+
+    def _trunk_node(self, ft, n, out):
+        fs, fc, A = int(ft.first_slot[n]), int(ft.first_child[n]), int(ft.n_children[n])
+        out.zero_()
+        out[:, torch.from_numpy(ft.action[fc:fc + A].astype(np.int64)).to(out.device)] = self.trunk[fs:fs + A, :ft.R].T
+
+    # ---- state
+    def state_dict(self):
+        return {"rows": self.rows.cpu(), "keys": self.keys.cpu(), "pos_hand": self.pos_hand.cpu(), "trunk": self.trunk.cpu(),
+                "iso": self.iso, "actions": self.actions, "fingerprint": self.fingerprint, "spec_id": self.spec_id}
+
+    @classmethod
+    def from_state(cls, state, device=None):
+        dev = _require_cuda(device)
+        return cls(*(state[k].to(dev) for k in ("rows", "keys", "pos_hand", "trunk")), state["iso"], state["actions"],
+                   state["fingerprint"], state["spec_id"])
+
+
+def _packed_actions(ft, st):
+    """discrete action of every post-deal local node (as a child) in 4 bits per node, board 0 of `ft`"""
+    act = 0
+    for i in range(1, st["n_local"]):
+        a = int(ft.action[st["node_base"][i] + st["node_k"][i]])
+        assert 0 <= a < 16
+        act |= a << (4 * i)
+    return act

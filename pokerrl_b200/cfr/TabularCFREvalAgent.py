@@ -1,7 +1,12 @@
 """Tabular CFR `EvalAgent` (SURVEY.md §8f N1): a concrete `EvalAgentBase` backed by the average-strategy table of a
 `pokerrl_b200.cfr` solver, so that the solver's result can be handed to the evaluators (`LocalBRMaster`) and stored /
 restored (`store_to_disk` / `load_from_disk`).  The reference ships no concrete tabular agent (EvalAgentBase.py is
-abstract); the query contract is `StrategyFiller._fill_with_agent_policy` (StrategyFiller.py:88-116)."""
+abstract); the query contract is `StrategyFiller._fill_with_agent_policy` (StrategyFiller.py:88-116).
+
+Solvers of the board engine (Flop5Holdem, pokerrl_b200.board_engine) hold no slot table: their agent keeps the strength-ordered
+rows, class keys and position -> hand tables (board_engine.BoardPolicyTables, about 8.2 GB of rows + 290 MB for the full
+game) and answers for any Flop5Holdem PublicTree - any board spec, either engine - with one kernel launch
+(prl_board_policy_query)."""
 import numpy as np
 
 from pokerrl_b200 import _native as nat
@@ -42,6 +47,7 @@ class TabularCFREvalAgent(EvalAgentBase):
     def __init__(self, t_prof, mode=None, device=None):
         super().__init__(t_prof=t_prof, mode=mode or self.EVAL_MODE_AVG, device=device)
         self._table = None  # float32 [n_slots, R]: rows in the flat tree's slot order
+        self._board = None  # board_engine.BoardPolicyTables of a board-engine solver
         self._n_actions = self.env_bldr.N_ACTIONS
 
     def update_weights(self, weights_for_eval_agent):
@@ -52,21 +58,29 @@ class TabularCFREvalAgent(EvalAgentBase):
             weights_for_eval_agent, fp = weights_for_eval_agent
         self._table = np.ascontiguousarray(weights_for_eval_agent, dtype=np.float32)
         self._fingerprint = fp
+        self._board = None
 
     @classmethod
     def from_cfr(cls, t_prof, cfr, tree_idx=0):
         agent = cls(t_prof=t_prof)
         solver = cfr.solvers[tree_idx]
+        if getattr(solver, "ft", None) is None and hasattr(solver, "ft1"):  # board engine: no slot table
+            from pokerrl_b200.board_engine import BoardPolicyTables
+            agent._board = BoardPolicyTables.from_solver(solver)
+            agent._fingerprint = (agent._board.fingerprint, agent._board.spec_id)
+            return agent
         agent.update_weights((average_strategy_table(solver), tree_fingerprint(solver.ft)))
         return agent
 
     def can_compute_mode(self):
-        return self._table is not None
+        return self._table is not None or self._board is not None
 
     def get_a_probs_for_each_hand(self):
         """[RANGE_SIZE, N_ACTIONS] with the node's probabilities at its allowed actions, 0 elsewhere"""
         node = self._node
         ft = node.tree.flat
+        if self._board is not None:
+            return self._board.answer_node(ft, node.idx, self._n_actions)
         if getattr(self, "_fingerprint", None) is not None and tree_fingerprint(ft) != self._fingerprint:
             raise ValueError("this agent's table was computed on a different public tree (stack / bet set / slot order): "
                              "build one agent per evaluated tree (TabularCFREvalAgent.from_cfr(..., tree_idx=...))")
@@ -79,6 +93,8 @@ class TabularCFREvalAgent(EvalAgentBase):
         """all decision nodes at once: [n_decision, R, N_ACTIONS] on the tree's device (one scatter of the table rows)"""
         import torch
         ft = tree.flat
+        if self._board is not None:
+            return self._board.answer_tree(ft, self._n_actions)
         if getattr(self, "_fingerprint", None) is not None and tree_fingerprint(ft) != self._fingerprint:
             raise ValueError("this agent's table was computed on a different public tree")
         dev = tree.dtree.device
@@ -92,8 +108,14 @@ class TabularCFREvalAgent(EvalAgentBase):
         return out
 
     def _state_dict(self):
-        return {"table": self._table, "fingerprint": getattr(self, "_fingerprint", None)}
+        """board engine: CPU tensors (the full game's rows are about 8.2 GB)"""
+        return {"table": self._table, "fingerprint": getattr(self, "_fingerprint", None),
+                "board": None if self._board is None else self._board.state_dict()}
 
     def _load_state_dict(self, state):
         self._table = state["table"]
         self._fingerprint = state.get("fingerprint")
+        self._board = None
+        if state.get("board") is not None:  # back onto the device
+            from pokerrl_b200.board_engine import BoardPolicyTables
+            self._board = BoardPolicyTables.from_state(state["board"], self.device)

@@ -921,6 +921,115 @@ __global__ void board_permute_kernel(const unsigned char* __restrict__ tables, i
 }
 
 // =====================================================================================================================
+// An agent's answers from its strength-ordered tables, for boards it may hold only as suit-isomorphism classes.  One CTA per
+// query board: canonical key -> class (binary search over the agent's sorted keys) -> out[d][h][action] in natural hand
+// order for the board's decision nodes.  The canonical key is the minimum over the 24 suit permutations s of the sorted cards
+// s(c) = rank * 4 + s[suit] packed base 64 (holdem_boards.canonical_boards); the permutation used is the FIRST minimal one in
+// itertools.permutations order, since a class's rows are suit-symmetric only up to rounding.  Hand h on the query board is
+// answered by the class's row entry of hand s(h) on the representative.
+// =====================================================================================================================
+__constant__ int8_t c_suit_perm[24][4] = {
+    {0, 1, 2, 3}, {0, 1, 3, 2}, {0, 2, 1, 3}, {0, 2, 3, 1}, {0, 3, 1, 2}, {0, 3, 2, 1}, {1, 0, 2, 3}, {1, 0, 3, 2},
+    {1, 2, 0, 3}, {1, 2, 3, 0}, {1, 3, 0, 2}, {1, 3, 2, 0}, {2, 0, 1, 3}, {2, 0, 3, 1}, {2, 1, 0, 3}, {2, 1, 3, 0},
+    {2, 3, 0, 1}, {2, 3, 1, 0}, {3, 0, 1, 2}, {3, 0, 2, 1}, {3, 1, 0, 2}, {3, 1, 2, 0}, {3, 2, 0, 1}, {3, 2, 1, 0}};
+
+// decision nodes of the compiled shape, ascending local id (the columns of out_index)
+constexpr int kNDec = 6;
+constexpr int dec_node(int d) {
+    int n = 0;
+    for (int i = 0; i < ShapeFHP::N; ++i)
+        if (ShapeFHP::kind(i) <= 1 && ShapeFHP::n_children(i) > 0 && n++ == d) return i;
+    return -1;
+}
+static_assert(dec_node(kNDec - 1) >= 0 && dec_node(kNDec) == -1, "decision nodes of the compiled shape");
+
+__device__ __forceinline__ int hand_index(int c1, int c2) {  // c1 < c2, LUT_HOLE_CARDS_2_IDX order
+    return c1 * (2 * kDeck - 1 - c1) / 2 + (c2 - c1 - 1);
+}
+
+__global__ void __launch_bounds__(256) policy_query_kernel(const float* __restrict__ rows, const long long* __restrict__ keys,
+                                                           const int16_t* __restrict__ pos_hand, int n_cls, int iso,
+                                                           const int8_t* __restrict__ boards, const int32_t* __restrict__ out_index,
+                                                           unsigned long long act, int n_actions, float* __restrict__ out,
+                                                           int* __restrict__ miss) {
+    __shared__ short s_pos[kRange];  // hand on the representative -> strength position
+    __shared__ long long s_key[24];
+    __shared__ int s_perm, s_cls;
+    const int q = blockIdx.x, tid = threadIdx.x;
+    int cards[kBoardCards];
+    uint64_t bm = 0;
+#pragma unroll
+    for (int k = 0; k < kBoardCards; ++k) {
+        cards[k] = boards[(size_t)q * kBoardCards + k];
+        bm |= 1ull << cards[k];
+    }
+    if (tid < 24) {
+        const int s = iso ? tid : 0;
+        int m[kBoardCards];
+#pragma unroll
+        for (int k = 0; k < kBoardCards; ++k) m[k] = (cards[k] >> 2) * 4 + c_suit_perm[s][cards[k] & 3];
+#pragma unroll
+        for (int i = 1; i < kBoardCards; ++i)
+#pragma unroll
+            for (int j = i; j > 0; --j)
+                if (m[j] < m[j - 1]) {
+                    const int t = m[j];
+                    m[j] = m[j - 1];
+                    m[j - 1] = t;
+                }
+        long long key = 0;
+#pragma unroll
+        for (int k = 0; k < kBoardCards; ++k) key = key * 64 + m[k];
+        s_key[tid] = key;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int best = 0;
+        if (iso)
+            for (int s = 1; s < 24; ++s)
+                if (s_key[s] < s_key[best]) best = s;  // strict: the first minimal permutation
+        const long long k = s_key[best];
+        int lo = 0, hi = n_cls;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (keys[mid] < k) lo = mid + 1;
+            else hi = mid;
+        }
+        s_perm = best;
+        s_cls = (lo < n_cls && keys[lo] == k) ? lo : -1;
+        if (s_cls < 0) atomicExch(miss, 1);
+    }
+    for (int h = tid; h < kRange; h += blockDim.x) s_pos[h] = -1;
+    __syncthreads();
+    const int cls = s_cls, sp = s_perm;
+    if (cls >= 0)
+        for (int i = tid; i < kLive; i += blockDim.x) s_pos[pos_hand[(size_t)cls * kLive + i]] = (short)i;
+    __syncthreads();
+    const float* crow = rows + (size_t)(cls < 0 ? 0 : cls) * ShapeFHP::rows * kLdb;
+    for (int h = tid; h < kRange; h += blockDim.x) {
+        int c1 = 0;
+        while (hand_index(c1 + 1, c1 + 2) <= h) ++c1;  // first card: the largest c1 whose hands start at or before h
+        const int c2 = h - hand_index(c1, c1 + 1) + c1 + 1;
+        int pos = -1;
+        if (cls >= 0 && !(((bm >> c1) | (bm >> c2)) & 1ull)) {
+            const int m1 = (c1 >> 2) * 4 + c_suit_perm[sp][c1 & 3], m2 = (c2 >> 2) * 4 + c_suit_perm[sp][c2 & 3];
+            pos = s_pos[hand_index(min(m1, m2), max(m1, m2))];
+        }
+#pragma unroll
+        for (int d = 0; d < kNDec; ++d) {
+            const int oi = out_index[(size_t)q * kNDec + d];
+            if (oi < 0) continue;
+            float* o = out + ((size_t)oi * kRange + h) * n_actions;
+            for (int a = 0; a < n_actions; ++a) o[a] = 0.0f;
+            if (pos < 0) continue;  // blocked hand (or a board the agent does not hold): all zero
+            const int n = dec_node(d), fc = ShapeFHP::first_child(n);
+            for (int c = fc; c < fc + ShapeFHP::n_children(n); ++c)
+                o[(act >> (4 * c)) & 0xF] = crow[(size_t)ShapeFHP::row_of(c) * kLdb + pos];
+        }
+    }
+}
+
+// =====================================================================================================================
 // The pre-deal trunk in ONE launch (one CTA): chance-node rows from the fixed-point sums (integer sum over the suit
 // permutations), fold terminals, value backup, and - update form - regrets / matching / average of seat p's trunk nodes and
 // its new reach rows; evaluation form: values + best response of both seats and the root exploitability.  Same statements as
@@ -1284,6 +1393,23 @@ extern "C" int prl_board_permute(const prl_board_game_t* g, int rows_per_board, 
         (const unsigned char*)g->tables, g->n_boards, rows_per_board, row_src, row_dst, sorted_tab, natural_tab, ld, to_natural);
     prl::count_launch();
     return prl::check(cudaGetLastError(), "prl_board_permute");
+}
+
+extern "C" int prl_board_policy_query(const float* rows, const int64_t* keys, const int16_t* pos_hand, int n_cls, int iso,
+                                      const int8_t* boards, int n_boards, const int32_t* out_index, uint64_t actions, int n_actions,
+                                      float* out, int32_t* miss, prl_stream_t stream) {
+    if (n_boards <= 0) return 0;
+    if (!rows || !keys || !pos_hand || n_cls <= 0 || !boards || !out_index || !out || !miss)
+        return prl::fail("prl_board_policy_query: missing buffers");
+    if (n_actions < 1 || n_actions > 16) return prl::fail("prl_board_policy_query: 1..16 actions");
+    for (int c = 1; c < ShapeFHP::N; ++c)
+        if (ShapeFHP::kind(ShapeFHP::parent(c)) <= 1 && (int)((actions >> (4 * c)) & 0xF) >= n_actions)
+            return prl::fail("prl_board_policy_query: an action id is out of range");
+    policy_query_kernel<<<n_boards, 256, 0, (cudaStream_t)stream>>>(rows, reinterpret_cast<const long long*>(keys), pos_hand, n_cls,
+                                                                    iso, boards, out_index, (unsigned long long)actions, n_actions, out,
+                                                                    reinterpret_cast<int*>(miss));
+    prl::count_launch();
+    return prl::check(cudaGetLastError(), "prl_board_policy_query");
 }
 
 // Trunk of seat p's half-iteration (eval == 0) or of an evaluation of both seats (eval != 0) in one launch; see prl_trunk_t.

@@ -1,6 +1,11 @@
 """Exact best-response evaluator for any `EvalAgentBase` (`PokerRL/eval/br/LocalBRMaster.py:11-80`): one HBM-resident
 `PublicTree` per evaluation stack size; `fill_with_agent_policy` -> reach pass -> value pass with BR on the GPU ->
-`root.exploitability * EV_NORMALIZER` averaged over the two seats."""
+`root.exploitability * EV_NORMALIZER` averaged over the two seats.
+
+Games the board engine supports (Flop5Holdem; PRL_ENGINE unset) are evaluated by `board_engine.BoardPolicyEvaluator`
+instead: the agent is queried chunk by chunk over the boards, so memory is bounded by the chunk, not by the game (a
+PublicTree of the full game would need about 104 GB).  board_spec (extension, like CFRBase's): the boards of the chance layer;
+default = the game's suit-isomorphism classes."""
 import copy
 
 from pokerrl_b200.eval._.EvaluatorMasterBase import EvaluatorMasterBase
@@ -9,14 +14,24 @@ from pokerrl_b200.rl.base_cls.TrainingProfileBase import get_env_builder
 
 
 class LocalBRMaster(EvaluatorMasterBase):
-    def __init__(self, t_prof, chief_handle, eval_agent_cls, device=None):
+    def __init__(self, t_prof, chief_handle, eval_agent_cls, device=None, board_spec=None):
         super().__init__(t_prof=t_prof, eval_env_bldr=get_env_builder(t_prof=t_prof), chief_handle=chief_handle,
                          eval_type="BR")
         self._env_bldr = get_env_builder(t_prof=t_prof)
         assert self._env_bldr.N_SEATS == 2
         self._eval_agent = eval_agent_cls(t_prof=t_prof)
+        from pokerrl_b200 import board_engine
+        env_cls = self._env_bldr.env_cls
+        if all(board_engine.supports(env_cls, self._env_bldr.args_for_stack(s), "CFRPlus") for s in t_prof.eval_stack_sizes):
+            self._game_trees = [board_engine.BoardPolicyEvaluator(self._env_bldr, stack_size=s, board_spec=board_spec, device=device)
+                                for s in t_prof.eval_stack_sizes]
+            for gt in self._game_trees:
+                print("Tree with stack size", gt.stack_size, "has", gt.n_nodes - 1, "nodes out of which", gt.n_nonterm - 1,
+                      "are non-terminal.")
+            return
         self._game_trees = [PublicTree(env_bldr=self._env_bldr, stack_size=stack_size, stop_at_street=None,
-                                       put_out_new_round_after_limit=True, is_debugging=t_prof.DEBUGGING, device=device)
+                                       put_out_new_round_after_limit=True, is_debugging=t_prof.DEBUGGING, device=device,
+                                       board_spec=board_spec)
                             for stack_size in t_prof.eval_stack_sizes]
         for gt in self._game_trees:
             gt.build_tree()
@@ -46,7 +61,10 @@ class LocalBRMaster(EvaluatorMasterBase):
 
     def _compute_br_heads_up(self, stack_size_idx, iter_nr=None, do_export_tree=True):
         gt = self._game_trees[stack_size_idx]
+        norm = self._env_bldr.env_cls.EV_NORMALIZER
+        if not isinstance(gt, PublicTree):  # board engine
+            e = gt.evaluate(self._eval_agent)
+            return float(e[0]) * norm, float(e[1]) * norm
         gt.fill_with_agent_policy(agent=self._eval_agent)
         gt.compute_ev()
-        norm = self._env_bldr.env_cls.EV_NORMALIZER
         return float(gt.root.exploitability[0]) * norm, float(gt.root.exploitability[1]) * norm

@@ -198,6 +198,24 @@ class PublicTree:
         self._has_reach = self._has_ev = False
         self.root = NodeView(self, 0)
 
+    def build_structure(self):
+        """The flat tree and a device handle only: no node vectors, no strength tables.  Enough to query an agent
+        (agent_strategy_table with an explicit `out`); the board engine's policy evaluation builds one per chunk of boards."""
+        from types import SimpleNamespace
+        from pokerrl_b200.solver import _require_cuda
+        args = self._env_bldr.args_for_stack(self._stack_size)
+        self.flat = FlatTree(self._env_bldr.env_cls, args, stop_at_street=self._stop_at_street_arg, board_spec=self._board_spec)
+        R = self.flat.R
+        self.dtree = SimpleNamespace(device=_require_cuda(self._device),
+                                     ld=R if self.flat.rules.N_HOLE_CARDS == 1 else -(-R // 4) * 4)
+        self.bufs = self.ops = None
+        self.modes = [nat.STRAT_UNIFORM64, nat.STRAT_UNIFORM64]
+        self._slot_maps = None
+        self._cache = {}
+        self._root_expl = None
+        self._has_reach = self._has_ev = False
+        self.root = NodeView(self, 0)
+
     # ---- strategy filling (StrategyFiller.py:17-46)
     def fill_uniform_random(self):
         self.modes = [nat.STRAT_UNIFORM64, nat.STRAT_UNIFORM64]
@@ -230,9 +248,21 @@ class PublicTree:
         return np.nonzero((ft.kind <= KIND_P1) & (ft.first_child >= 0))[0]
 
     def fill_with_agent_policy(self, agent):
-        """StrategyFiller._fill_with_agent_policy (:88-116).  Agents that answer for the whole tree at once
-        (`get_a_probs_for_public_tree(tree)` -> device float32 [n_decision, R, N_ACTIONS]) are filled by ONE device gather;
-        others are queried node by node like the reference does."""
+        """StrategyFiller._fill_with_agent_policy (:88-116): the agent's strategy table (agent_strategy_table), then the
+        reach pass."""
+        tab = self.agent_strategy_table(agent)
+        if isinstance(tab, torch.Tensor):
+            self.modes = [nat.STRAT_F32, nat.STRAT_F32]
+            self.update_reach_probs()
+        else:
+            self.set_strategy_table(tab)
+
+    def agent_strategy_table(self, agent, out=None):
+        """The agent's strategy table, one row per slot.  Agents that answer for the whole tree at once
+        (`get_a_probs_for_public_tree(tree)` -> device float32 [n_decision, R, N_ACTIONS]) are gathered by ONE device launch
+        into `out` (float32 [n_slots, ld] on the tree's device; default: the tree's `strat` buffer), which is returned.  Others
+        are queried node by node like the reference does; the host table [n_slots, R] is returned (float64 if any answer
+        was float64, else float32)."""
         ft = self.flat
         batched = getattr(agent, "get_a_probs_for_public_tree", None)
         probs = batched(self) if batched is not None else None
@@ -240,9 +270,11 @@ class PublicTree:
             import ctypes as C
             from pokerrl_b200.solver import _on, _stream
             dev = self.dtree.device
+            out = self.bufs.strat if out is None else out
             probs = torch.as_tensor(probs).to(device=dev, dtype=torch.float32).contiguous()
             dec = self.decision_nodes()
             assert probs.shape[0] == dec.size and probs.shape[1] == ft.R, probs.shape
+            assert out.shape[0] >= ft.n_slots and out.shape[1] == self.dtree.ld and out.dtype == torch.float32, out.shape
             if getattr(self, "_slot_maps", None) is None:
                 dec_idx = np.full(ft.n_nodes, -1, np.int64)
                 dec_idx[dec] = np.arange(dec.size)
@@ -252,11 +284,9 @@ class PublicTree:
             d_of, a_of = self._slot_maps
             with _on(dev):
                 nat.call("prl_gather_agent_policy", C.c_void_p(probs.data_ptr()), int(probs.shape[2]), C.c_void_p(d_of.data_ptr()),
-                         C.c_void_p(a_of.data_ptr()), ft.n_slots, ft.R, self.dtree.ld, C.c_void_p(self.bufs.strat.data_ptr()),
+                         C.c_void_p(a_of.data_ptr()), ft.n_slots, ft.R, self.dtree.ld, C.c_void_p(out.data_ptr()),
                          _stream(dev))
-            self.modes = [nat.STRAT_F32, nat.STRAT_F32]
-            self.update_reach_probs()
-            return
+            return out
         rows, dt = np.zeros((ft.n_slots, ft.R)), None
         for n in np.nonzero((ft.kind <= KIND_P1) & (ft.first_child >= 0))[0]:
             node = NodeView(self, n)
@@ -264,7 +294,7 @@ class PublicTree:
             a_probs = np.asarray(agent.get_a_probs_for_each_hand())
             dt = a_probs.dtype if dt is None else np.promote_types(dt, a_probs.dtype)
             rows[ft.first_slot[n]:ft.first_slot[n] + ft.n_children[n]] = a_probs[:, node.allowed_actions].T
-        self.set_strategy_table(rows if dt == np.float64 else rows.astype(np.float32))
+        return rows if dt == np.float64 else rows.astype(np.float32)
 
     def update_reach_probs(self):
         self.ops.reach_pass(self.modes)

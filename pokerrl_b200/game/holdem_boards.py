@@ -83,6 +83,26 @@ def canonical_boards(boards, n_suits=4):
     return reps, counts.astype(np.int32)
 
 
+def canonical_keys(boards, n_suits=4):
+    """(key int64 [n], perm int64 [n]): each board's class key - the minimum over the suit permutations of its sorted cards
+    packed base 64, as in canonical_boards - and the index, in itertools.permutations order, of the FIRST permutation that
+    attains it (the rule by which prl_board_policy_query maps a board's hands onto its class representative's)."""
+    boards = np.asarray(boards, dtype=np.int64)
+    rank, suit = boards // n_suits, boards % n_suits
+    best, arg = None, None
+    for s, sp in enumerate(permutations(range(n_suits))):
+        m = np.sort(rank * n_suits + np.array(sp)[suit], axis=1)
+        key = np.zeros(m.shape[0], np.int64)
+        for i in range(boards.shape[1]):
+            key = key * 64 + m[:, i]
+        if best is None:
+            best, arg = key, np.zeros(key.shape[0], np.int64)
+        else:
+            lower = key < best  # strict: an equal key later in the order does not replace the first
+            best, arg = np.where(lower, key, best), np.where(lower, s, arg)
+    return best, arg
+
+
 class BoardSpec:
     """Boards dealt at the (single) chance layer of a two-card game + their weights."""
 
