@@ -28,8 +28,9 @@ typedef void* prl_stream_t; /* cudaStream_t */
 /* bumped whenever a struct below changes; prl_abi_version() returns the value the library was built with
    (2: prl_tree_t gained board_hand_rec / node_rec2 / work_rec2 / level_nfold; 3: board engine, legacy LUT natives;
     4: prl_board_sweep / prl_board_trunk take the algorithm; prl_tree_t gained the all-in terminals of two-card games: level_nallin / allin_nodes / allin_pot / allin_tiles /
-    allin_partial; 5: prl_board_update_cfrp / prl_board_avg_flush; 6: prl_board_policy_query) */
-#define PRL_ABI_VERSION 6
+    allin_partial; 5: prl_board_update_cfrp / prl_board_avg_flush; 6: prl_board_policy_query; 7: second board-engine shape,
+    prl_board_layout / prl_board_rows / prl_board_policy_query take the shape) */
+#define PRL_ABI_VERSION 7
 
 /* node kinds (game/_/tree/_/nodes.py:8-62 + ValueFiller.py:34-62) */
 enum {
@@ -227,7 +228,9 @@ int prl_board_order_tables(const int32_t* ranks, int n_boards, int n_range, int 
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Board-resident CFR+ engine (csrc/cfr_board.cu) for two-card games with ONE chance layer whose post-deal subtree has
- * the compiled shape (Flop5Holdem, PokerRL/game/games.py:222-254: 15 nodes per board).  Replaces, for the post-deal
+ * a compiled shape (Flop5Holdem, PokerRL/game/games.py:222-254: 15 nodes per board for stacks of 901 chips and more, 9 nodes
+ * for 301 to 900 chips, where the flop's pot-size bet is all-in).  Every entry point that takes a prl_board_game_t picks the
+ * shape its kind / parent / first_child / n_children match and fails on a descriptor that matches none.  Replaces, for the post-deal
  * levels, ValueFiller.compute_cf_values_heads_up (ValueFiller.py:21-158), StrategyFiller._update_reach_probs
  * (StrategyFiller.py:118-146) and the regret / matching / averaging of CFRPlus.py:37-87: one persistent kernel walks
  * (board, seat) units with the subtree in registers / shared memory.  Table rows of a board are stored in the board's
@@ -259,10 +262,15 @@ typedef struct {
 } prl_board_game_t;
 
 /* out[8] = {n_live, ldb, blob bytes per board, byte offset of the int16 hand ids, byte offset of the card rows,
- *           live cards, padded card-row length, nodes of the compiled shape} */
-int prl_board_layout(int32_t* out);
+ *           live cards, padded card-row length, nodes of the compiled shape}.  shape = a descriptor whose kind / parent /
+ * first_child / n_children name a compiled shape (only those fields are read), or NULL: the per-board blob layout alone, out[7] = 0. */
+int prl_board_layout(const prl_board_game_t* shape, int32_t* out);
 int prl_board_grid(void);                              /* default CTA count on the current device */
-int prl_board_shape_ok(const prl_board_game_t* g);     /* 1 iff kind / parent / first_child / n_children match */
+int prl_board_shape_ok(const prl_board_game_t* g);     /* 1 iff kind / parent / first_child / n_children match a compiled shape */
+/* The board-major row layout of the shape that `shape` names (as in prl_board_layout, not NULL): row_of = int32[16], the table
+ * row of local node i (a child of a decision node) on board 0, -1 for the others; *rows_per_board = rows of one board
+ * (14 / 8 for the 15- / 9-node shape). */
+int prl_board_rows(const prl_board_game_t* shape, int32_t* row_of, int32_t* rows_per_board);
 
 /* ranks = DEVICE int32[n_boards][1326] (prl_hand_rank_boards), board_mask = DEVICE uint64[n_boards] -> blob */
 int prl_board_build_tables(const int32_t* ranks, const uint64_t* board_mask, const int8_t* hand_cards, int n_boards,
@@ -331,18 +339,19 @@ int prl_board_permute(const prl_board_game_t* g, int rows_per_board, const int64
                       float* sorted_tab, float* natural_tab, int ld, int to_natural, prl_stream_t stream);
 
 /* An agent's answers from its strength-ordered tables (EvalAgentBase.get_a_probs_for_each_hand for the post-deal decision nodes
- * of n_boards boards, one CTA per board).  The agent: rows = DEVICE float[n_cls][14][ldb] in the board-major row layout of
- * prl_board_rows, keys = DEVICE int64[n_cls] ascending class keys, pos_hand = DEVICE int16[n_cls][n_live] (the hand ids of the
+ * of n_boards boards, one CTA per board).  shape = the agent's post-deal shape (as in prl_board_layout, not NULL).  The agent:
+ * rows = DEVICE float[n_cls][rows_per_board][ldb] in the board-major row layout of prl_board_rows for that shape,
+ * keys = DEVICE int64[n_cls] ascending class keys, pos_hand = DEVICE int16[n_cls][n_live] (the hand ids of the
  * representative's blob: strength position -> hand).  A key packs the five sorted cards base 64 (holdem_boards.canonical_boards);
  * iso != 0: the query board's key is the minimum over the 24 suit permutations, the FIRST minimal one in itertools.permutations
  * order maps its hands onto the representative's; iso == 0: the board's own key.  boards = DEVICE int8[n_boards][5];
- * out_index = DEVICE int32[n_boards][6]: for the compiled shape's decision nodes in ascending local id, the index d of the node in
- * out (-1: not wanted); actions = discrete action of local node i in bits 4i..4i+3.  Writes out[d][h][a] (DEVICE float
+ * out_index = DEVICE int32[n_boards][n_dec] (n_dec = 6 / 4 decision nodes in the 15- / 9-node shape): for the shape's decision
+ * nodes in ascending local id, the index d of the node in out (-1: not wanted); actions = discrete action of local node i in bits 4i..4i+3.  Writes out[d][h][a] (DEVICE float
  * [.][1326][n_actions], natural hand order): the row of the child with action a at hand h's position, 0 for blocked hands and
  * for actions the node does not allow.  A board whose key the agent does not hold sets *miss (DEVICE int32) to 1. */
-int prl_board_policy_query(const float* rows, const int64_t* keys, const int16_t* pos_hand, int n_cls, int iso,
-                           const int8_t* boards, int n_boards, const int32_t* out_index, uint64_t actions, int n_actions,
-                           float* out, int32_t* miss, prl_stream_t stream);
+int prl_board_policy_query(const prl_board_game_t* shape, const float* rows, const int64_t* keys, const int16_t* pos_hand,
+                           int n_cls, int iso, const int8_t* boards, int n_boards, const int32_t* out_index, uint64_t actions,
+                           int n_actions, float* out, int32_t* miss, prl_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * 7-card Hold'em hand evaluation (replaces lib_hand_eval.so; int32 strength, higher = better, identical encoding incl.

@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("PRL_LIB_PATH") or os.path.join(_HERE, "lib", "libpoke
 # enums of include/pokerrl_b200.h
 KIND_P0, KIND_P1, KIND_CHANCE, KIND_FOLD, KIND_SHOWDOWN, KIND_SHOWDOWN_ALLIN = range(6)
 ALGO_VANILLA, ALGO_CFR_PLUS, ALGO_LINEAR = 0, 1, 2
-ABI_VERSION = 6  # include/pokerrl_b200.h: PRL_ABI_VERSION
+ABI_VERSION = 7  # include/pokerrl_b200.h: PRL_ABI_VERSION
 STRAT_F32, STRAT_UNIFORM64, STRAT_AVG_F64, STRAT_AVG_SUM, STRAT_AVG_F32 = range(5)
 
 
@@ -135,9 +135,9 @@ def lib():
     for f in ("prl_allin_equity_accumulate", "prl_allin_equity_finish", "prl_allin_values"):
         getattr(L, f).restype = C.c_int
     gp = C.POINTER(PrlBoardGame)
-    L.prl_board_layout.argtypes = [C.POINTER(C.c_int32)]
+    L.prl_board_layout.argtypes = [gp, C.POINTER(C.c_int32)]
     L.prl_board_grid.argtypes = []
-    L.prl_board_rows.argtypes = [C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    L.prl_board_rows.argtypes = [gp, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
     L.prl_board_rows.restype = C.c_int
     L.prl_board_shape_ok.argtypes = [gp]
     L.prl_board_build_tables.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
@@ -151,8 +151,8 @@ def lib():
     L.prl_board_trunk.argtypes = [gp, C.POINTER(PrlTrunk), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                   C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_void_p]
     L.prl_board_trunk.restype = C.c_int
-    L.prl_board_policy_query.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
-                                         C.c_uint64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.prl_board_policy_query.argtypes = [gp, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                         C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     for f in ("prl_board_layout", "prl_board_grid", "prl_board_shape_ok", "prl_board_build_tables", "prl_board_sweep",
               "prl_board_update_cfrp", "prl_board_avg_flush", "prl_board_collect", "prl_board_permute", "prl_board_policy_query"):
         getattr(L, f).restype = C.c_int

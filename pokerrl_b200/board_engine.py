@@ -25,9 +25,10 @@ SRC_REGRET, SRC_AVG, SRC_AVG_SUM = 0, 1, 2
 ALGOS = {"VanillaCFR": nat.ALGO_VANILLA, "CFRPlus": nat.ALGO_CFR_PLUS, "LinearCFR": nat.ALGO_LINEAR}
 
 
-def board_layout():
+def board_layout(g=None):
+    """prl_board_layout: the per-board blob layout; n_local = nodes of the compiled shape the descriptor `g` names (0 without)"""
     out = (C.c_int32 * 8)()
-    nat.call("prl_board_layout", out)
+    nat.call("prl_board_layout", C.byref(g) if g is not None else None, out)
     return dict(n_live=out[0], ldb=out[1], blob=out[2], sh_off=out[3], rows_off=out[4], live_cards=out[5],
                 row_pad=out[6], n_local=out[7])
 
@@ -37,7 +38,8 @@ def _stream(dev):
 
 
 def supports(game_cls, env_args, algo):
-    """True iff the game's abstract tree is one pre-deal trunk + one chance layer + the compiled post-deal shape"""
+    """True iff the game's abstract tree is one pre-deal trunk + one chance layer + a compiled post-deal shape (Flop5Holdem:
+    stacks of 301 chips and more; at 300 and below the preflop raise is all-in and there is no post-deal betting)"""
     if algo not in ALGOS or game_cls.RULES.N_HOLE_CARDS != 2 or game_cls.RULES.N_CARDS_IN_DECK != 52:
         return False
     if game_cls.RULES.N_FLOP_CARDS != 5 or os.environ.get("PRL_ENGINE", "board") != "board":
@@ -63,6 +65,13 @@ def _fill_shape(g, st):
     for i in range(st["n_local"]):
         g.kind[i], g.parent[i], g.first_child[i] = st["kind"][i], st["parent"][i], st["first_child"][i]
         g.n_children[i], g.acted_last[i], g.pot[i] = st["n_children"][i], st["acted_last"][i], st["pot"][i]
+
+
+def shape_rows(g):
+    """(row_of[16], rows_per_board) of the compiled shape the descriptor `g` names (prl_board_rows): the board-major row layout"""
+    row_of, rpb = (C.c_int32 * 16)(), C.c_int32(0)
+    nat.call("prl_board_rows", C.byref(g), row_of, C.byref(rpb))
+    return list(row_of), int(rpb.value)
 
 
 def board_mask(boards):
@@ -105,17 +114,16 @@ def board_game(st, rules, n_boards, ld, n_sym, grid=0):
     dec = [i for i in range(n_local) if st["kind"][i] <= 1]
     rows_per_board = sum(st["n_children"][i] for i in dec)
     # board-major rows: everything a (board, seat) unit touches is contiguous - row(i, j) = j * rows_per_board + row_of[i]
-    row_of, rpb = (C.c_int32 * 16)(), C.c_int32(0)
-    nat.call("prl_board_rows", row_of, C.byref(rpb))
-    assert rpb.value == rows_per_board
+    row_of, rpb = shape_rows(g)
+    assert rpb == rows_per_board
     local_rows = {}  # local child node -> (row on board 0, stride per board)
     for i in range(n_local):
         g.row0[i], g.row_m[i] = -1, 0
     for d in dec:
         for a in range(st["n_children"][d]):
             c = st["first_child"][d] + a
-            g.row0[c], g.row_m[c] = row_of[c], rpb.value
-            local_rows[c] = (int(row_of[c]), rpb.value)
+            g.row0[c], g.row_m[c] = row_of[c], rpb
+            local_rows[c] = (int(row_of[c]), rpb)
     g.grid = int(grid) if grid else int(nat.lib().prl_board_grid())
     return g, rows_per_board, local_rows
 
@@ -571,7 +579,8 @@ class BoardPolicyEvaluator(_BoardTrunk):
         bytes_per_board = blob (15 392) + strength-ordered rows (rows_per_board * 1088 * 4)
                           + slot-table rows (rows_per_board * ld * 4) + the batched answers (n_dec * 1326 * N_ACTIONS * 4)
                           + hand ranks (1326 * 4)
-    (Flop5Holdem: 14 rows, ld 1328, 6 decision nodes, 3 actions: 245 KB per board), plus the trunk and the chance sums.
+    (Flop5Holdem, ld 1328, 3 actions: 245 KB per board at stacks of 901 chips and more - 14 rows, 6 decision nodes -, 158 KB
+    at 301 to 900 chips - 8 rows, 4 decision nodes), plus the trunk and the chance sums.
     Default chunk = min(65 536, n_boards, free device memory / 2 / bytes_per_board)."""
 
     MAX_CHUNK = 65536
@@ -701,12 +710,14 @@ class BoardPolicyTables:
       pos_hand  int16   [n_cls, 1081]                    strength position -> hand, cut from the boards' tables
       trunk     float32 [n_trunk_slots, ld]              trunk rows, natural hand order
     iso: the spec holds suit-isomorphism classes (queries are canonicalised), else raw boards.  Answers for the decision nodes
-    of any flat tree of the game (any board spec, either engine) through prl_board_policy_query."""
+    of any flat tree of the game (any board spec, either engine) through prl_board_policy_query.  The post-deal shape is that of
+    the game and stack the tables were computed on: rows_per_board = rows.shape[0] / n_cls tells it apart."""
 
     def __init__(self, rows, keys, pos_hand, trunk, iso, actions, fingerprint, spec_id):
         self.rows, self.keys, self.pos_hand, self.trunk = rows, keys, pos_hand, trunk
         self.iso, self.actions, self.fingerprint, self.spec_id = bool(iso), int(actions), fingerprint, spec_id
         self.n_cls = int(keys.shape[0])
+        self.rows_per_board = int(rows.shape[0]) // self.n_cls
 
     @classmethod
     def from_solver(cls, s):
@@ -772,13 +783,18 @@ class BoardPolicyTables:
         if abstract_fingerprint(ft) != self.fingerprint:
             raise ValueError("this agent's tables were computed on a different betting tree (game / stack / bet set)")
 
-    def _query(self, boards, out_index, out, n_actions):
+    def _query(self, st, boards, out_index, out, n_actions):
+        g = nat.PrlBoardGame()
+        _fill_shape(g, st)
+        if shape_rows(g)[1] != self.rows_per_board:
+            raise ValueError("this agent's tables hold %d rows per board, the queried tree's post-deal shape has %d"
+                             % (self.rows_per_board, shape_rows(g)[1]))
         dev = out.device
         miss = torch.zeros(1, dtype=torch.int32, device=dev)
         t_b = torch.from_numpy(np.ascontiguousarray(boards, np.int8)).to(dev)
         t_i = torch.from_numpy(np.ascontiguousarray(out_index, np.int32)).to(dev)
         with torch.cuda.device(dev):
-            nat.call("prl_board_policy_query", C.c_void_p(self.rows.data_ptr()), C.c_void_p(self.keys.data_ptr()),
+            nat.call("prl_board_policy_query", C.byref(g), C.c_void_p(self.rows.data_ptr()), C.c_void_p(self.keys.data_ptr()),
                      C.c_void_p(self.pos_hand.data_ptr()), self.n_cls, int(self.iso), C.c_void_p(t_b.data_ptr()), int(t_b.shape[0]),
                      C.c_void_p(t_i.data_ptr()), self.actions, n_actions, C.c_void_p(out.data_ptr()), C.c_void_p(miss.data_ptr()),
                      _stream(dev))
@@ -803,7 +819,7 @@ class BoardPolicyTables:
         idx = np.full((nb, len(locs)), -1, np.int64)
         for d, i in enumerate(locs):
             idx[:, d] = dec_idx[st["node_base"][i] + J * st["node_m"][i] + st["node_k"][i]]
-        self._query(ft.board_spec.boards, idx, out, n_actions)
+        self._query(st, ft.board_spec.boards, idx, out, n_actions)
         return out
 
     def answer_node(self, ft, n, n_actions):
@@ -821,7 +837,7 @@ class BoardPolicyTables:
             if st["node_base"][i] + j * st["node_m"][i] + st["node_k"][i] == n:
                 idx[0, d] = 0
         assert (idx == 0).sum() == 1, "not a post-deal decision node"
-        self._query(ft.board_spec.boards[j:j + 1], idx, out, n_actions)
+        self._query(st, ft.board_spec.boards[j:j + 1], idx, out, n_actions)
         return out[0].cpu().numpy()
 
     def _trunk_node(self, ft, n, out):

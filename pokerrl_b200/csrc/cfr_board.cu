@@ -84,8 +84,8 @@ constexpr int kThreads = 384;  // 12 warps; 3 strength positions per thread (3 *
 constexpr int kPerThread = 3;
 constexpr int kWarps = kThreads / 32;
 
-// ---- compiled shape of the post-deal subtree (breadth-first; Flop5Holdem with pot-size raises, stacks that allow the
-//      full raise sequence).  The host checks the game's abstract tree against these arrays.
+// ---- compiled shapes of the post-deal subtree (breadth-first; Flop5Holdem with pot-size raises).  The host checks the game's
+//      abstract tree against these arrays and picks the shape it matches.
 // per-node tables packed 4 bits per node (value + 1): a lookup is a shift, never a local-memory array
 struct Nodes15 {
     int v[15];
@@ -97,16 +97,13 @@ constexpr unsigned long long pack_nodes(Nodes15 t) {
 }
 constexpr int unpack_node(unsigned long long t, int i) { return (int)((t >> (4 * i)) & 0xF) - 1; }
 
-struct ShapeFHP {
-    static constexpr int N = 15;
-    static constexpr unsigned long long kKind = pack_nodes({{1, 0, 0, 4, 1, 3, 4, 1, 3, 4, 0, 3, 4, 3, 4}});
-    static constexpr unsigned long long kParent = pack_nodes({{-1, 0, 0, 1, 1, 2, 2, 2, 4, 4, 4, 7, 7, 10, 10}});
-    static constexpr unsigned long long kFirstChild = pack_nodes({{1, 3, 5, -1, 8, -1, -1, 11, -1, -1, 13, -1, -1, -1, -1}});
-    static constexpr unsigned long long kNChildren = pack_nodes({{2, 2, 3, 0, 3, 0, 0, 2, 0, 0, 2, 0, 0, 0, 0}});
-    static constexpr int kind(int i) { return unpack_node(kKind, i); }
-    static constexpr int parent(int i) { return unpack_node(kParent, i); }
-    static constexpr int first_child(int i) { return unpack_node(kFirstChild, i); }
-    static constexpr int n_children(int i) { return unpack_node(kNChildren, i); }
+// what every shape derives from its four node arrays (SH::N, kKind, kParent, kFirstChild, kNChildren)
+template <class SH>
+struct ShapeOps {
+    static constexpr int kind(int i) { return unpack_node(SH::kKind, i); }
+    static constexpr int parent(int i) { return unpack_node(SH::kParent, i); }
+    static constexpr int first_child(int i) { return unpack_node(SH::kFirstChild, i); }
+    static constexpr int n_children(int i) { return unpack_node(SH::kNChildren, i); }
     // index of terminal i among the showdown / fold vectors
     static constexpr int vec_index(int i) {
         int n = 0;
@@ -115,36 +112,76 @@ struct ShapeFHP {
     }
     static constexpr int count(int k) {
         int n = 0;
-        for (int i = 0; i < N; ++i) n += (kind(i) == k);
+        for (int i = 0; i < SH::N; ++i) n += (kind(i) == k);
         return n;
     }
-    static constexpr int n_sd = 5, n_fold = 4;
     // table rows of one board: the rows of seat 0's decision nodes first, then seat 1's, children in breadth-first order
     static constexpr int rows_of_seat(int p) {
         int n = 0;
-        for (int i = 1; i < N; ++i) n += (kind(parent(i)) == p);
+        for (int i = 1; i < SH::N; ++i) n += (kind(parent(i)) == p);
         return n;
     }
-    static constexpr int rows = 14;
     static constexpr int row_of(int c) {  // c = child of a decision node
         const int p = kind(parent(c));
         int n = (p == 0) ? 0 : rows_of_seat(0);
         for (int k = 1; k < c; ++k) n += (kind(parent(k)) == p);
         return n;
     }
+    // decision nodes, ascending local id (the columns of prl_board_policy_query's out_index)
+    static constexpr int n_dec() {
+        int n = 0;
+        for (int i = 0; i < SH::N; ++i) n += (kind(i) <= 1 && n_children(i) > 0);
+        return n;
+    }
+    static constexpr int dec_node(int d) {
+        int n = 0;
+        for (int i = 0; i < SH::N; ++i)
+            if (kind(i) <= 1 && n_children(i) > 0 && n++ == d) return i;
+        return -1;
+    }
 };
-static_assert(ShapeFHP::count(4) == ShapeFHP::n_sd && ShapeFHP::count(3) == ShapeFHP::n_fold, "shape");
-// Reach of the OPPONENT of seat P at fold terminal f as a combination of its reach at the showdown terminals (strategies sum
-// to one, own nodes copy the reach): x_fold[f] = sum_v coef(P, f, v) * x_sd[v].  Every linear functional of the fold vectors
-// (their card-row sums) follows from the showdown vectors' at no cost.  tools/fold_relations.py derives the table.
-struct FoldLinFHP {
-    static constexpr int coef(int P, int f, int v) {
+
+// Stacks of 901 chips and more: the flop bet, the pot-size raise and the all-in re-raise all fit.
+// fold_coef: reach of the OPPONENT of seat P at fold terminal f as a combination of its reach at the showdown terminals
+// (strategies sum to one, own nodes copy the reach): x_fold[f] = sum_v fold_coef(P, f, v) * x_sd[v].  Every linear functional
+// of the fold vectors (their card-row sums) follows from the showdown vectors' at no cost.  tools/fold_relations.py derives
+// the tables of both shapes.
+struct ShapeFHP : ShapeOps<ShapeFHP> {
+    static constexpr int N = 15;
+    static constexpr unsigned long long kKind = pack_nodes({{1, 0, 0, 4, 1, 3, 4, 1, 3, 4, 0, 3, 4, 3, 4}});
+    static constexpr unsigned long long kParent = pack_nodes({{-1, 0, 0, 1, 1, 2, 2, 2, 4, 4, 4, 7, 7, 10, 10}});
+    static constexpr unsigned long long kFirstChild = pack_nodes({{1, 3, 5, -1, 8, -1, -1, 11, -1, -1, 13, -1, -1, -1, -1}});
+    static constexpr unsigned long long kNChildren = pack_nodes({{2, 2, 3, 0, 3, 0, 0, 2, 0, 0, 2, 0, 0, 0, 0}});
+    static constexpr int n_sd = 5, n_fold = 4;
+    static constexpr int rows = 14;
+    static constexpr int fold_coef(int P, int f, int v) {
         constexpr int c[2][4][5] = {{{0, 1, 0, 0, 0}, {1, 0, -1, 0, -1}, {0, 1, 0, -1, 0}, {0, 0, 0, 0, 1}},
                                     {{1, -1, 1, -1, 0}, {0, 0, 1, 0, 0}, {0, 0, 0, 1, 0}, {0, 0, 1, 0, -1}}};
         return c[P][f][v];
     }
 };
-static_assert(ShapeFHP::rows_of_seat(0) + ShapeFHP::rows_of_seat(1) == ShapeFHP::rows, "shape");
+
+// Stacks of 301 to 900 chips: the flop's pot-size bet is all-in, so the player facing it may only fold or call.
+struct ShapeFHPShort : ShapeOps<ShapeFHPShort> {
+    static constexpr int N = 9;
+    static constexpr unsigned long long kKind = pack_nodes({{1, 0, 0, 4, 1, 3, 4, 3, 4}});
+    static constexpr unsigned long long kParent = pack_nodes({{-1, 0, 0, 1, 1, 2, 2, 4, 4}});
+    static constexpr unsigned long long kFirstChild = pack_nodes({{1, 3, 5, -1, 7, -1, -1, -1, -1}});
+    static constexpr unsigned long long kNChildren = pack_nodes({{2, 2, 2, 0, 2, 0, 0, 0, 0}});
+    static constexpr int n_sd = 3, n_fold = 2;
+    static constexpr int rows = 8;
+    static constexpr int fold_coef(int P, int f, int v) {
+        constexpr int c[2][2][3] = {{{0, 1, 0}, {1, 0, -1}}, {{1, -1, 1}, {0, 0, 1}}};
+        return c[P][f][v];
+    }
+};
+
+template <class SH>
+constexpr bool shape_consistent() {
+    return SH::count(4) == SH::n_sd && SH::count(3) == SH::n_fold && SH::rows_of_seat(0) + SH::rows_of_seat(1) == SH::rows &&
+           SH::N <= 15 && SH::n_fold % 2 == 0;  // P2a splits the fold vectors evenly over two groups
+}
+static_assert(shape_consistent<ShapeFHP>() && shape_consistent<ShapeFHPShort>(), "shape");
 
 template <int I, int N, class F>
 __device__ __forceinline__ void static_for(F&& f) {
@@ -161,24 +198,29 @@ __device__ __forceinline__ void static_for_down(F&& f) {  // N-1 .. I
     }
 }
 
-// ---- shared memory carve-up (bytes)
-constexpr int kNVec = ShapeFHP::n_sd + ShapeFHP::n_fold;                   // 9 terminal vectors
-constexpr int kSOff = 0;                                                    // float S[9][1088]
-constexpr int kErOff = kSOff + kNVec * kLdb * 4;                            // float Er[5][47*47]
+// ---- shared memory carve-up of the sweep (bytes; ShapeFHP: 9 terminal vectors, 5 of them showdowns, 4 folds)
 constexpr int kErVec = kLiveCards * kErStride;                              // 2209 floats per showdown vector
-constexpr int kErBytes = ((ShapeFHP::n_sd * kErVec * 4) + 15) & ~15;
-constexpr int kBlobOff = kErOff + kErBytes;                                 // 2 x (rec + hand ids)
-constexpr int kRowIdxOff = kBlobOff + 2 * kBlobA;                           // card rows (single buffer)
-constexpr int kCsOff = kRowIdxOff + kRowIdxBytes;                           // float cs[4][48] per-card sums of the fold vectors
-constexpr int kCsdOff = kCsOff + ShapeFHP::n_fold * kRowPad * 4;            // double csd[4][48]: the same sums before rounding
-constexpr int kMiscOff = kCsdOff + ShapeFHP::n_fold * kRowPad * 8;          // double wsum[5][16], wexc[5][16]; float tf[8]
-constexpr int kMiscBytes = (5 * 16 + 5 * 16) * 8 + 8 * 4;
-constexpr int kRowTotOff = kMiscOff + kMiscBytes;                           // double rowtot[5][48]: card-row totals of the showdown vectors
-constexpr int kRowTotBytes = ShapeFHP::n_sd * kRowPad * 8;
-constexpr int kBarOff = kRowTotOff + kRowTotBytes;                          // 3 mbarriers
-constexpr int kSmemBytes = kBarOff + 32;
-static_assert(kBlobOff % 16 == 0 && kRowIdxOff % 16 == 0 && kCsdOff % 8 == 0 && kMiscOff % 8 == 0 && kRowTotOff % 8 == 0 && kBarOff % 8 == 0, "alignment");
-static_assert(2 * (kSmemBytes + 1024) <= 233472, "two CTAs per SM (228 KB of shared memory per H100 SM)");
+template <class SH>
+struct SweepSmem {
+    static constexpr int kNVec = SH::n_sd + SH::n_fold;                     // terminal vectors
+    static constexpr int kSOff = 0;                                         // float S[kNVec][1088]
+    static constexpr int kErOff = kSOff + kNVec * kLdb * 4;                 // float Er[n_sd][47*47]
+    static constexpr int kErBytes = ((SH::n_sd * kErVec * 4) + 15) & ~15;
+    static constexpr int kBlobOff = kErOff + kErBytes;                      // 2 x (rec + hand ids)
+    static constexpr int kRowIdxOff = kBlobOff + 2 * kBlobA;                // card rows (single buffer)
+    static constexpr int kCsOff = kRowIdxOff + kRowIdxBytes;                // float cs[n_fold][48] per-card sums of the fold vectors
+    static constexpr int kCsdOff = kCsOff + SH::n_fold * kRowPad * 4;       // double csd[n_fold][48]: the same sums before rounding
+    static constexpr int kMiscOff = kCsdOff + SH::n_fold * kRowPad * 8;     // double wsum[n_sd][16], wexc[n_sd][16]; float tf[8]
+    static constexpr int kMiscBytes = (SH::n_sd * 16 + SH::n_sd * 16) * 8 + 8 * 4;
+    static constexpr int kRowTotOff = kMiscOff + kMiscBytes;                // double rowtot[n_sd][48]: card-row totals of the showdown vectors
+    static constexpr int kRowTotBytes = SH::n_sd * kRowPad * 8;
+    static constexpr int kBarOff = kRowTotOff + kRowTotBytes;               // 3 mbarriers
+    static constexpr int kSmemBytes = kBarOff + 32;
+    static_assert(kBlobOff % 16 == 0 && kRowIdxOff % 16 == 0 && kCsdOff % 8 == 0 && kMiscOff % 8 == 0 && kRowTotOff % 8 == 0 &&
+                      kBarOff % 8 == 0, "alignment");
+    static_assert(2 * (kSmemBytes + 1024) <= 233472, "two CTAs per SM (228 KB of shared memory per H100 SM)");
+    static_assert(SH::n_fold <= 8, "tf[8]");
+};
 
 struct SweepArgs {
     prl_board_game_t g;
@@ -285,7 +327,7 @@ __device__ __forceinline__ void st_stream(float* p, float v) { __stcs(p, v); }
 // =====================================================================================================================
 // The sweep kernel.  P = seat whose values are computed; EVAL = false: CFR+ update of seat P (regrets, average);
 // EVAL = true: values and best-response values of seat P under the strategies selected by src_own / src_opp.
-// Table rows of board j: [j][14][1088] floats, rows ShapeFHP::row_of(child); everything a unit touches is contiguous.
+// Table rows of board j: [j][SH::rows][1088] floats, rows SH::row_of(child); everything a unit touches is contiguous.
 // =====================================================================================================================
 // DEFER (Vanilla / Linear CFR, update form): regrets are not clipped, and the average is the reach-weighted SUM of
 // strategies (VanillaCFR.py:54-60, LinearCFR.py:53-59) with the seat's reach under its NEW strategy - which includes its
@@ -299,24 +341,25 @@ __device__ __forceinline__ void st_stream(float* p, float v) { __stcs(p, v); }
 template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true>
 __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArgs a) {
     static_assert(!(EVAL && DEFER) && (!P1ONLY || DEFER) && (AVG || (!EVAL && !DEFER)), "variants");
+    using M = SweepSmem<SH>;
+    constexpr int NSD = SH::n_sd, NF = SH::n_fold;
     extern __shared__ __align__(128) unsigned char smem[];
-    float* S = reinterpret_cast<float*>(smem + kSOff);
-    float* Er = reinterpret_cast<float*>(smem + kErOff);
-    float* cs = reinterpret_cast<float*>(smem + kCsOff);
-    double* csd = reinterpret_cast<double*>(smem + kCsdOff);
-    double* wsum = reinterpret_cast<double*>(smem + kMiscOff);  // [5][16] warp totals of the main scans
-    double* wexc = wsum + 5 * 16;                                // [5][16] exclusive prefix of the warp totals - total / 2
-    float* tf = reinterpret_cast<float*>(wexc + 5 * 16);         // [8]     totals of the fold vectors
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kBarOff);  // [0], [1]: blob A buffers; [2]: card rows
-    const int16_t* rowidx = reinterpret_cast<const int16_t*>(smem + kRowIdxOff);
-    double* rowtot = reinterpret_cast<double*>(smem + kRowTotOff);  // [5][48]
+    float* S = reinterpret_cast<float*>(smem + M::kSOff);
+    float* Er = reinterpret_cast<float*>(smem + M::kErOff);
+    float* cs = reinterpret_cast<float*>(smem + M::kCsOff);
+    double* csd = reinterpret_cast<double*>(smem + M::kCsdOff);
+    double* wsum = reinterpret_cast<double*>(smem + M::kMiscOff);  // [NSD][16] warp totals of the main scans
+    double* wexc = wsum + NSD * 16;                                 // [NSD][16] exclusive prefix of the warp totals - total / 2
+    float* tf = reinterpret_cast<float*>(wexc + NSD * 16);          // [8]       totals of the fold vectors
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + M::kBarOff);  // [0], [1]: blob A buffers; [2]: card rows
+    const int16_t* rowidx = reinterpret_cast<const int16_t*>(smem + M::kRowIdxOff);
+    double* rowtot = reinterpret_cast<double*>(smem + M::kRowTotOff);  // [NSD][48]
     constexpr bool kLin = kVFoldLin && !EVAL;  // evaluation may read average-strategy rows, which sum to one only up to rounding
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const prl_board_game_t& G = a.g;
     const int nb = G.n_boards;
     constexpr int OPP = 1 - P;
-    constexpr int NSD = SH::n_sd, NF = SH::n_fold;
     constexpr int ROWS = SH::rows;
     constexpr int OWN0 = (P == 0) ? 0 : SH::rows_of_seat(0);      // first table row of the seat / of the opponent
     constexpr int OPP0 = (P == 0) ? SH::rows_of_seat(0) : 0;
@@ -335,7 +378,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
     // private chance-sum accumulators of this CTA (global, L2-resident): [2][kRange] int64
     long long* wp = reinterpret_cast<long long*>(G.w_private) + (size_t)blockIdx.x * 2 * kRange;
     for (int h = tid; h < 2 * kRange; h += kThreads) wp[h] = 0;
-    for (int v = 0; v < kNVec; ++v)
+    for (int v = 0; v < M::kNVec; ++v)
         for (int i = kLive + tid; i < kLdb; i += kThreads) S[v * kLdb + i] = 0.0f;  // incl. the always-zero slot
     if (tid == 0) {
         mbar_init(&bars[0], 1);
@@ -369,10 +412,10 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
     };
     if (tid == 0 && j < nb) {  // first board's tables
         mbar_expect_tx(&bars[0], kBlobA);
-        bulk_g2s(smem + kBlobOff, blob_g + (size_t)j * kBlobBytes, kBlobA, &bars[0]);
+        bulk_g2s(smem + M::kBlobOff, blob_g + (size_t)j * kBlobBytes, kBlobA, &bars[0]);
         if (!P1ONLY) {
             mbar_expect_tx(&bars[2], kRowIdxBytes);
-            bulk_g2s(smem + kRowIdxOff, blob_g + (size_t)j * kBlobBytes + kBlobA, kRowIdxBytes, &bars[2]);
+            bulk_g2s(smem + M::kRowIdxOff, blob_g + (size_t)j * kBlobBytes + kBlobA, kRowIdxBytes, &bars[2]);
         }
         if constexpr (kPfPhase) prefetch_opp(j);
         else prefetch_rows(j);
@@ -398,14 +441,14 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
 
     for (int it = 0; j < nb; j += gridDim.x, ++it) {
         const int buf = it & 1;
-        const unsigned char* blob = smem + kBlobOff + buf * kBlobA;
+        const unsigned char* blob = smem + M::kBlobOff + buf * kBlobA;
         const uint64_t* rec = reinterpret_cast<const uint64_t*>(blob);
         const int16_t* sh = reinterpret_cast<const int16_t*>(blob + kRecBytes);
         const int jn = j + gridDim.x;
         stamp(it, 0);
         if (tid == 0 && jn < nb) {  // next board: records + hand ids into the other buffer (free since the last barrier), rows into L2
             mbar_expect_tx(&bars[buf ^ 1], kBlobA);
-            bulk_g2s(smem + kBlobOff + (buf ^ 1) * kBlobA, blob_g + (size_t)jn * kBlobBytes, kBlobA, &bars[buf ^ 1]);
+            bulk_g2s(smem + M::kBlobOff + (buf ^ 1) * kBlobA, blob_g + (size_t)jn * kBlobBytes, kBlobA, &bars[buf ^ 1]);
             if constexpr (!kPfPhase) prefetch_rows(jn);
         }
         const float prob = __ldg(G.board_prob + j);
@@ -482,12 +525,14 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
         // ------------------------------------------------------------------------------------------ P2a: card rows
         // quad (live card lc, lane q): entries [12 q, 12 q + 12) of the card's row in strength order.  Showdown vectors:
         // centred exclusive prefix sums Er[v][lc][k] = (mass of the k weakest hands holding the card) - half the row's mass;
-        // fold vectors: the row's mass cs[f][lc].  Two groups of 47 quads share the nine vectors (SD 0-2 + fold 0-1 | SD 3-4 +
-        // fold 2-3); the other threads start on the main scans, which only read S as well.
+        // fold vectors: the row's mass cs[f][lc].  Two groups of 47 quads share the terminal vectors (ShapeFHP: SD 0-2 + fold
+        // 0-1 | SD 3-4 + fold 2-3; ShapeFHPShort: SD 0-1 + fold 0 | SD 2 + fold 1); the other threads start on the main scans,
+        // which only read S as well.
         mbar_wait(&bars[2], it & 1);
         float a0[NSD], a1[NSD], a2[NSD];
         double pre[NSD];
         constexpr int kQuadThreads = kLiveCards * 4;  // 188
+        constexpr int kSdSplit = (NSD + 1) / 2, kFoldSplit = NF / 2;  // first vector of the second group
         if (warp < (2 * kQuadThreads + 31) / 32) {   // whole warps (the quad shuffles name every lane)
             const int grp = (tid >= kQuadThreads) ? 1 : 0;
             const int t = tid - grp * kQuadThreads;
@@ -500,7 +545,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
             int idx[kRowSeg];
 #pragma unroll
             for (int e = 0; e < kRowSeg; ++e) idx[e] = (pk[e >> 1] >> ((e & 1) * 16)) & 0xffffu;
-            const int v_lo = grp ? 3 : 0, v_hi = grp ? NSD : 3;
+            const int v_lo = grp ? kSdSplit : 0, v_hi = grp ? NSD : kSdSplit;
 #pragma unroll 1
             for (int v = v_lo; v < v_hi; ++v) {
                 const float* Sv = S + v * kLdb;
@@ -533,7 +578,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
                     if (row_live && q * kRowSeg + e < kErStride) row[kVErT ? e * kErStride : e] = off + inc[e];
             }
 #pragma unroll 1
-            for (int f = 2 * grp; f < (kLin ? 0 : 2 * grp + 2); ++f) {  // kLin: nothing to gather for the fold vectors
+            for (int f = kFoldSplit * grp; f < (kLin ? 0 : kFoldSplit * grp + kFoldSplit); ++f) {  // kLin: nothing to gather for the fold vectors
                 const float* Sv = S + (NSD + f) * kLdb;
                 double run = 0.0;  // double: the fold value subtracts these sums from the total (cancellation)
 #pragma unroll
@@ -591,19 +636,18 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
         stamp(it, 2);
         if (tid == 0 && jn < nb) {
             mbar_expect_tx(&bars[2], kRowIdxBytes);
-            bulk_g2s(smem + kRowIdxOff, blob_g + (size_t)jn * kBlobBytes + kBlobA, kRowIdxBytes, &bars[2]);
+            bulk_g2s(smem + M::kRowIdxOff, blob_g + (size_t)jn * kBlobBytes + kBlobA, kRowIdxBytes, &bars[2]);
             if constexpr (kPfPhase) prefetch_opp(jn);
         }
         // card-row sums cs[f][card] and total tf[f] of fold vector f (total = half the sum of its card rows): from the gathered
-        // sums csd, or - kLin - as the combination FoldLinFHP of the showdown vectors' row totals
+        // sums csd, or - kLin - as the combination SH::fold_coef of the showdown vectors' row totals
         auto fold_finish = [&](auto F) {
             constexpr int f = decltype(F)::value;
             double c0 = 0.0, c1 = 0.0;
             if constexpr (kLin) {
-                static_assert(std::is_same<SH, ShapeFHP>::value, "FoldLinFHP belongs to ShapeFHP");
                 static_for<0, NSD>([&](auto V) {
                     constexpr int v = decltype(V)::value;
-                    constexpr int cf = FoldLinFHP::coef(P, f, v);
+                    constexpr int cf = SH::fold_coef(P, f, v);
                     if constexpr (cf != 0) {
                         const double r0 = (lane < kLiveCards) ? rowtot[v * kRowPad + lane] : 0.0;
                         const double r1 = (lane + 32 < kLiveCards) ? rowtot[v * kRowPad + lane + 32] : 0.0;
@@ -767,7 +811,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
         // next unit's P1 inputs: requested before the barrier below, consumed after it (the other table buffer is long there)
         if (jn < nb) {
             mbar_wait(&bars[buf ^ 1], ((it + 1) >> 1) & 1);
-            p1_load(jn, reinterpret_cast<const int16_t*>(smem + kBlobOff + (buf ^ 1) * kBlobA + kRecBytes));
+            p1_load(jn, reinterpret_cast<const int16_t*>(smem + M::kBlobOff + (buf ^ 1) * kBlobA + kRecBytes));
         }
         __syncthreads();  // B5: S / Er / tables of this board are free
         stamp(it, 5);
@@ -933,20 +977,13 @@ __constant__ int8_t c_suit_perm[24][4] = {
     {1, 2, 0, 3}, {1, 2, 3, 0}, {1, 3, 0, 2}, {1, 3, 2, 0}, {2, 0, 1, 3}, {2, 0, 3, 1}, {2, 1, 0, 3}, {2, 1, 3, 0},
     {2, 3, 0, 1}, {2, 3, 1, 0}, {3, 0, 1, 2}, {3, 0, 2, 1}, {3, 1, 0, 2}, {3, 1, 2, 0}, {3, 2, 0, 1}, {3, 2, 1, 0}};
 
-// decision nodes of the compiled shape, ascending local id (the columns of out_index)
-constexpr int kNDec = 6;
-constexpr int dec_node(int d) {
-    int n = 0;
-    for (int i = 0; i < ShapeFHP::N; ++i)
-        if (ShapeFHP::kind(i) <= 1 && ShapeFHP::n_children(i) > 0 && n++ == d) return i;
-    return -1;
-}
-static_assert(dec_node(kNDec - 1) >= 0 && dec_node(kNDec) == -1, "decision nodes of the compiled shape");
 
 __device__ __forceinline__ int hand_index(int c1, int c2) {  // c1 < c2, LUT_HOLE_CARDS_2_IDX order
     return c1 * (2 * kDeck - 1 - c1) / 2 + (c2 - c1 - 1);
 }
 
+// out_index[q][d], d < SH::n_dec(): the shape's decision nodes in ascending local id (SH::dec_node)
+template <class SH>
 __global__ void __launch_bounds__(256) policy_query_kernel(const float* __restrict__ rows, const long long* __restrict__ keys,
                                                            const int16_t* __restrict__ pos_hand, int n_cls, int iso,
                                                            const int8_t* __restrict__ boards, const int32_t* __restrict__ out_index,
@@ -955,6 +992,7 @@ __global__ void __launch_bounds__(256) policy_query_kernel(const float* __restri
     __shared__ short s_pos[kRange];  // hand on the representative -> strength position
     __shared__ long long s_key[24];
     __shared__ int s_perm, s_cls;
+    constexpr int kNDec = SH::n_dec();
     const int q = blockIdx.x, tid = threadIdx.x;
     int cards[kBoardCards];
     uint64_t bm = 0;
@@ -1005,7 +1043,7 @@ __global__ void __launch_bounds__(256) policy_query_kernel(const float* __restri
     if (cls >= 0)
         for (int i = tid; i < kLive; i += blockDim.x) s_pos[pos_hand[(size_t)cls * kLive + i]] = (short)i;
     __syncthreads();
-    const float* crow = rows + (size_t)(cls < 0 ? 0 : cls) * ShapeFHP::rows * kLdb;
+    const float* crow = rows + (size_t)(cls < 0 ? 0 : cls) * SH::rows * kLdb;
     for (int h = tid; h < kRange; h += blockDim.x) {
         int c1 = 0;
         while (hand_index(c1 + 1, c1 + 2) <= h) ++c1;  // first card: the largest c1 whose hands start at or before h
@@ -1022,9 +1060,9 @@ __global__ void __launch_bounds__(256) policy_query_kernel(const float* __restri
             float* o = out + ((size_t)oi * kRange + h) * n_actions;
             for (int a = 0; a < n_actions; ++a) o[a] = 0.0f;
             if (pos < 0) continue;  // blocked hand (or a board the agent does not hold): all zero
-            const int n = dec_node(d), fc = ShapeFHP::first_child(n);
-            for (int c = fc; c < fc + ShapeFHP::n_children(n); ++c)
-                o[(act >> (4 * c)) & 0xF] = crow[(size_t)ShapeFHP::row_of(c) * kLdb + pos];
+            const int n = SH::dec_node(d), fc = SH::first_child(n);
+            for (int c = fc; c < fc + SH::n_children(n); ++c)
+                o[(act >> (4 * c)) & 0xF] = crow[(size_t)SH::row_of(c) * kLdb + pos];
         }
     }
 }
@@ -1207,20 +1245,32 @@ __global__ void __launch_bounds__(kTrunkThreads) trunk_kernel(const prl_trunk_t 
     }
 }
 
+template <class SH>
 bool shape_matches(const prl_board_game_t* g) {
-    if (g->n_local != ShapeFHP::N) return false;
-    for (int i = 0; i < ShapeFHP::N; ++i)
-        if (g->kind[i] != ShapeFHP::kind(i) || g->parent[i] != ShapeFHP::parent(i) || g->first_child[i] != ShapeFHP::first_child(i) ||
-            g->n_children[i] != ShapeFHP::n_children(i))
+    if (g->n_local != SH::N) return false;
+    for (int i = 0; i < SH::N; ++i)
+        if (g->kind[i] != SH::kind(i) || g->parent[i] != SH::parent(i) || g->first_child[i] != SH::first_child(i) ||
+            g->n_children[i] != SH::n_children(i))
             return false;
     return true;
 }
 
-// the table layout the kernel compiles in: row(i, j) = j * 14 + row_of(i)
+// the table layout the kernel compiles in: row(i, j) = j * SH::rows + row_of(i)
+template <class SH>
 bool layout_matches(const prl_board_game_t* g) {
-    for (int i = 1; i < ShapeFHP::N; ++i)
-        if (g->row0[i] != ShapeFHP::row_of(i) || g->row_m[i] != ShapeFHP::rows) return false;
+    for (int i = 1; i < SH::N; ++i)
+        if (g->row0[i] != SH::row_of(i) || g->row_m[i] != SH::rows) return false;
     return true;
+}
+
+// f(SH{}) for the compiled shape whose kind / parent / first_child / n_children the descriptor holds; kNoShape if none does
+constexpr int kNoShape = -1000;
+template <class F>
+int with_shape(const prl_board_game_t* g, F&& f) {
+    if (!g) return kNoShape;
+    if (shape_matches<ShapeFHP>(g)) return f(ShapeFHP{});
+    if (shape_matches<ShapeFHPShort>(g)) return f(ShapeFHPShort{});
+    return kNoShape;
 }
 
 int default_grid() {
@@ -1236,9 +1286,10 @@ int default_grid() {
     return cached[dev];
 }
 
-template <int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true>
+template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true>
 int launch_sweep(const SweepArgs& a, int grid, cudaStream_t s) {
-    auto kern = board_sweep_kernel<ShapeFHP, P, EVAL, DEFER, P1ONLY, AVG>;
+    auto kern = board_sweep_kernel<SH, P, EVAL, DEFER, P1ONLY, AVG>;
+    constexpr int kSmemBytes = SweepSmem<SH>::kSmemBytes;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);  // per device: set every time
     if (e != cudaSuccess) return prl::check(e, "prl_board_sweep: shared memory opt-in");
     kern<<<grid, kThreads, kSmemBytes, s>>>(a);
@@ -1256,7 +1307,12 @@ void cfrp_weights(int iter, int delay, float* m_old, float* m_new) {
 
 }  // namespace
 
-extern "C" int prl_board_layout(int32_t* out) {
+extern "C" int prl_board_layout(const prl_board_game_t* shape, int32_t* out) {
+    int n_local = 0;
+    if (shape) {
+        n_local = with_shape(shape, [](auto sh) { return decltype(sh)::N; });
+        if (n_local == kNoShape) return prl::fail("prl_board_layout: the post-deal subtree has no compiled shape");
+    }
     out[0] = kLive;
     out[1] = kLdb;
     out[2] = kBlobBytes;
@@ -1264,19 +1320,25 @@ extern "C" int prl_board_layout(int32_t* out) {
     out[4] = kBlobA;               // offset of the card rows
     out[5] = kLiveCards;
     out[6] = kRowPad;
-    out[7] = ShapeFHP::N;
+    out[7] = n_local;
     return 0;
 }
 
 extern "C" int prl_board_grid(void) { return default_grid(); }
 
-extern "C" int prl_board_rows(int32_t* row_of, int32_t* rows_per_board) {
-    for (int i = 0; i < 16; ++i) row_of[i] = (i >= 1 && i < ShapeFHP::N) ? ShapeFHP::row_of(i) : -1;
-    *rows_per_board = ShapeFHP::rows;
-    return 0;
+extern "C" int prl_board_rows(const prl_board_game_t* shape, int32_t* row_of, int32_t* rows_per_board) {
+    const int rc = with_shape(shape, [&](auto sh) {
+        using SH = decltype(sh);
+        for (int i = 0; i < 16; ++i) row_of[i] = (i >= 1 && i < SH::N) ? SH::row_of(i) : -1;
+        *rows_per_board = SH::rows;
+        return 0;
+    });
+    return rc == kNoShape ? prl::fail("prl_board_rows: the post-deal subtree has no compiled shape") : rc;
 }
 
-extern "C" int prl_board_shape_ok(const prl_board_game_t* g) { return (g && shape_matches(g)) ? 1 : 0; }
+extern "C" int prl_board_shape_ok(const prl_board_game_t* g) {
+    return with_shape(g, [](auto) { return 1; }) == 1 ? 1 : 0;
+}
 
 extern "C" int prl_board_build_tables(const int32_t* ranks, const uint64_t* board_mask, const int8_t* hand_cards, int n_boards,
                                       void* blob, prl_stream_t stream) {
@@ -1293,9 +1355,10 @@ static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, 
     if (algo != PRL_ALGO_CFR_PLUS && algo != PRL_ALGO_VANILLA && algo != PRL_ALGO_LINEAR) return prl::fail("prl_board_sweep: bad algo");
     const bool defer = !eval && algo != PRL_ALGO_CFR_PLUS;
     if (p1_only && !defer) return prl::fail("prl_board_sweep: p1_only is the average flush of Vanilla / Linear CFR");
-    if (!g || !shape_matches(g)) return prl::fail("prl_board_sweep: the post-deal subtree does not have the compiled shape");
+    const int layout_ok = with_shape(g, [&](auto sh) { return layout_matches<decltype(sh)>(g) ? 1 : 0; });
+    if (layout_ok == kNoShape) return prl::fail("prl_board_sweep: the post-deal subtree has no compiled shape");
     if (g->n_range != kRange || g->n_deck != kDeck) return prl::fail("prl_board_sweep: 52-card deck / 1326 hands only");
-    if (!layout_matches(g)) return prl::fail("prl_board_sweep: row0 / row_m must be the board-major layout of prl_board_rows");
+    if (!layout_ok) return prl::fail("prl_board_sweep: row0 / row_m must be the board-major layout of prl_board_rows");
     if (p < 0 || p > 1) return prl::fail("prl_board_sweep: bad seat");
     if (!g->tables || !g->regret || !g->avg || !g->w_private || !g->w_total || !trunk_reach_opp)
         return prl::fail("prl_board_sweep: missing buffers");
@@ -1323,18 +1386,24 @@ static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, 
         a.sc[n] = (n < g->n_local) ? g->eq_const * g->pot[n] * 0.5f * (folder ? -1.0f : 1.0f) : 0.0f;
     }
     if (p1_only) {
-        const int rc1 = (p == 0) ? launch_sweep<0, false, true, true>(a, grid, s) : launch_sweep<1, false, true, true>(a, grid, s);
+        const int rc1 = with_shape(g, [&](auto sh) {
+            using SH = decltype(sh);
+            return (p == 0) ? launch_sweep<SH, 0, false, true, true>(a, grid, s) : launch_sweep<SH, 1, false, true, true>(a, grid, s);
+        });
         return rc1 ? rc1 : prl::check(cudaGetLastError(), "prl_board_sweep(flush)");
     }
     {   // the sums this launch produces: update -> w_total[0]; evaluation of seat p -> w_total[2p], w_total[2p + 1]
         char* base = reinterpret_cast<char*>(g->w_total) + (eval ? sizeof(long long) * 2 * p * kRange : 0);
         if (int e = prl::check(cudaMemsetAsync(base, 0, sizeof(long long) * (eval ? 2 : 1) * kRange, s), "prl_board_sweep: memset")) return e;
     }
-    int rc;
-    if (eval) rc = (p == 0) ? launch_sweep<0, true>(a, grid, s) : launch_sweep<1, true>(a, grid, s);
-    else if (defer) rc = (p == 0) ? launch_sweep<0, false, true>(a, grid, s) : launch_sweep<1, false, true>(a, grid, s);
-    else if (step) rc = (p == 0) ? launch_sweep<0, false>(a, grid, s) : launch_sweep<1, false>(a, grid, s);
-    else rc = (p == 0) ? launch_sweep<0, false, false, false, false>(a, grid, s) : launch_sweep<1, false, false, false, false>(a, grid, s);
+    const int rc = with_shape(g, [&](auto sh) {
+        using SH = decltype(sh);
+        if (eval) return (p == 0) ? launch_sweep<SH, 0, true>(a, grid, s) : launch_sweep<SH, 1, true>(a, grid, s);
+        if (defer) return (p == 0) ? launch_sweep<SH, 0, false, true>(a, grid, s) : launch_sweep<SH, 1, false, true>(a, grid, s);
+        if (step) return (p == 0) ? launch_sweep<SH, 0, false>(a, grid, s) : launch_sweep<SH, 1, false>(a, grid, s);
+        return (p == 0) ? launch_sweep<SH, 0, false, false, false, false>(a, grid, s)
+                        : launch_sweep<SH, 1, false, false, false, false>(a, grid, s);
+    });
     if (rc) return rc;
     return prl::check(cudaGetLastError(), "prl_board_sweep");
 }
@@ -1350,7 +1419,8 @@ extern "C" int prl_board_update_cfrp(const prl_board_game_t* g, int p, const flo
 }
 
 extern "C" int prl_board_avg_flush(const prl_board_game_t* g, int p, int due, int delay, prl_stream_t stream) {
-    if (!g || !shape_matches(g) || !layout_matches(g)) return prl::fail("prl_board_avg_flush: not the compiled shape / layout");
+    const int layout_ok = with_shape(g, [&](auto sh) { return layout_matches<decltype(sh)>(g) ? 1 : 0; });
+    if (layout_ok != 1) return prl::fail("prl_board_avg_flush: not a compiled shape / layout");
     if (p < 0 || p > 1) return prl::fail("prl_board_avg_flush: bad seat");
     if (due < delay) return prl::fail("prl_board_avg_flush: no averaging step before iteration delay");
     if (!g->regret || !g->avg) return prl::fail("prl_board_avg_flush: missing buffers");
@@ -1358,8 +1428,12 @@ extern "C" int prl_board_avg_flush(const prl_board_game_t* g, int p, int due, in
     float m_old, m_new;
     cfrp_weights(due, delay, &m_old, &m_new);
     cudaStream_t s = (cudaStream_t)stream;
-    if (p == 0) avg_flush_kernel<ShapeFHP, 0><<<g->n_boards, 256, 0, s>>>(g->regret, g->avg, m_old, m_new);
-    else avg_flush_kernel<ShapeFHP, 1><<<g->n_boards, 256, 0, s>>>(g->regret, g->avg, m_old, m_new);
+    with_shape(g, [&](auto sh) {
+        using SH = decltype(sh);
+        if (p == 0) avg_flush_kernel<SH, 0><<<g->n_boards, 256, 0, s>>>(g->regret, g->avg, m_old, m_new);
+        else avg_flush_kernel<SH, 1><<<g->n_boards, 256, 0, s>>>(g->regret, g->avg, m_old, m_new);
+        return 0;
+    });
     prl::count_launch();
     return prl::check(cudaGetLastError(), "prl_board_avg_flush");
 }
@@ -1388,6 +1462,8 @@ extern "C" int prl_board_collect(const prl_board_game_t* g, int n_arr, const int
 
 extern "C" int prl_board_permute(const prl_board_game_t* g, int rows_per_board, const int64_t* row_src, const int64_t* row_dst,
                                  float* sorted_tab, float* natural_tab, int ld, int to_natural, prl_stream_t stream) {
+    if (g && with_shape(g, [](auto) { return 0; }) == kNoShape)
+        return prl::fail("prl_board_permute: the post-deal subtree has no compiled shape");
     if (!g || g->n_boards <= 0 || rows_per_board <= 0) return 0;
     board_permute_kernel<<<g->n_boards * rows_per_board, 256, 0, (cudaStream_t)stream>>>(
         (const unsigned char*)g->tables, g->n_boards, rows_per_board, row_src, row_dst, sorted_tab, natural_tab, ld, to_natural);
@@ -1395,19 +1471,26 @@ extern "C" int prl_board_permute(const prl_board_game_t* g, int rows_per_board, 
     return prl::check(cudaGetLastError(), "prl_board_permute");
 }
 
-extern "C" int prl_board_policy_query(const float* rows, const int64_t* keys, const int16_t* pos_hand, int n_cls, int iso,
-                                      const int8_t* boards, int n_boards, const int32_t* out_index, uint64_t actions, int n_actions,
-                                      float* out, int32_t* miss, prl_stream_t stream) {
+extern "C" int prl_board_policy_query(const prl_board_game_t* shape, const float* rows, const int64_t* keys, const int16_t* pos_hand,
+                                      int n_cls, int iso, const int8_t* boards, int n_boards, const int32_t* out_index,
+                                      uint64_t actions, int n_actions, float* out, int32_t* miss, prl_stream_t stream) {
+    if (with_shape(shape, [](auto) { return 0; }) == kNoShape)
+        return prl::fail("prl_board_policy_query: the post-deal subtree has no compiled shape");
     if (n_boards <= 0) return 0;
     if (!rows || !keys || !pos_hand || n_cls <= 0 || !boards || !out_index || !out || !miss)
         return prl::fail("prl_board_policy_query: missing buffers");
     if (n_actions < 1 || n_actions > 16) return prl::fail("prl_board_policy_query: 1..16 actions");
-    for (int c = 1; c < ShapeFHP::N; ++c)
-        if (ShapeFHP::kind(ShapeFHP::parent(c)) <= 1 && (int)((actions >> (4 * c)) & 0xF) >= n_actions)
-            return prl::fail("prl_board_policy_query: an action id is out of range");
-    policy_query_kernel<<<n_boards, 256, 0, (cudaStream_t)stream>>>(rows, reinterpret_cast<const long long*>(keys), pos_hand, n_cls,
-                                                                    iso, boards, out_index, (unsigned long long)actions, n_actions, out,
-                                                                    reinterpret_cast<int*>(miss));
+    const int rc = with_shape(shape, [&](auto sh) {
+        using SH = decltype(sh);
+        for (int c = 1; c < SH::N; ++c)
+            if (SH::kind(SH::parent(c)) <= 1 && (int)((actions >> (4 * c)) & 0xF) >= n_actions)
+                return prl::fail("prl_board_policy_query: an action id is out of range");
+        policy_query_kernel<SH><<<n_boards, 256, 0, (cudaStream_t)stream>>>(rows, reinterpret_cast<const long long*>(keys), pos_hand,
+                                                                            n_cls, iso, boards, out_index, (unsigned long long)actions,
+                                                                            n_actions, out, reinterpret_cast<int*>(miss));
+        return 0;
+    });
+    if (rc) return rc;
     prl::count_launch();
     return prl::check(cudaGetLastError(), "prl_board_policy_query");
 }
@@ -1419,6 +1502,7 @@ extern "C" int prl_board_trunk(const prl_board_game_t* g, const prl_trunk_t* t, 
     if (algo != PRL_ALGO_CFR_PLUS && algo != PRL_ALGO_VANILLA && algo != PRL_ALGO_LINEAR) return prl::fail("prl_board_trunk: bad algo");
     const float rw = (algo == PRL_ALGO_LINEAR) ? (float)(iter + 1) : 1.0f;
     if (!g || !t || t->n_nodes < 1 || t->n_nodes > 8) return prl::fail("prl_board_trunk: 1..8 trunk nodes");
+    if (with_shape(g, [](auto) { return 0; }) == kNoShape) return prl::fail("prl_board_trunk: the post-deal subtree has no compiled shape");
     if (t->n_range != kRange || g->n_deck != kDeck) return prl::fail("prl_board_trunk: 52-card deck / 1326 hands only");
     if (eval && !out_expl) return prl::fail("prl_board_trunk: out_expl missing");
     for (int n = 0; n < t->n_nodes; ++n)

@@ -1,5 +1,5 @@
-"""Timing probe of the board engine on one GPU: python tools/board_probe.py [n_boards] [iterations] [grid]
-CUDA-event times of the iteration, of each form of the CFR+ update sweep and of the average flush (per launch, over many
+"""Timing probe of the board engine on one GPU: python tools/board_probe.py [n_boards] [iterations] [grid] [stack]
+(stack default 20000: the 15-node post-deal shape; 301 to 900: the 9-node one).  CUDA-event times of the iteration, of each form of the CFR+ update sweep and of the average flush (per launch, over many
 launches), and of the evaluation passes, with the bytes each form moves and the card it ran on."""
 import ctypes as C
 import json
@@ -20,8 +20,9 @@ from pokerrl_b200.game.holdem_boards import BoardSpec  # noqa: E402
 nb = int(sys.argv[1]) if len(sys.argv) > 1 else 20000
 iters = int(sys.argv[2]) if len(sys.argv) > 2 else 10
 grid = int(sys.argv[3]) if len(sys.argv) > 3 else 0
+stack = int(sys.argv[4]) if len(sys.argv) > 4 else 20000
 g = games.Flop5Holdem
-args = g.ARGS_CLS(n_seats=2, starting_stack_sizes_list=[20000, 20000], bet_sizes_list_as_frac_of_pot=[1.0])
+args = g.ARGS_CLS(n_seats=2, starting_stack_sizes_list=[stack, stack], bet_sizes_list_as_frac_of_pot=[1.0])
 t0 = time.perf_counter()
 spec = BoardSpec.full_game(g.RULES)
 if nb < spec.boards.shape[0]:
@@ -66,8 +67,10 @@ forms = {
                                  stream),
     "flush": lambda p: nat.call("prl_board_avg_flush", C.byref(s.g), p, t - 1, s.delay, stream),
 }
-row = s.L["ldb"] * 4
-bytes_per_board = {"defer": 21 * row + s.L["blob"], "paired": 35 * row + s.L["blob"], "flush": 21 * row}
+# a seat owns half of a board's rows: defer reads the opponent's and its own regrets and writes its own (3 halves), paired also
+# reads and writes its average (5 halves), flush reads its regrets and average and writes its average (3 halves)
+row, half = s.L["ldb"] * 4, s.rows_per_board // 2
+bytes_per_board = {"defer": 3 * half * row + s.L["blob"], "paired": 5 * half * row + s.L["blob"], "flush": 3 * half * row}
 times = {k: [] for k in forms}
 for rnd in range(3):
     for k, launch in forms.items():
@@ -85,4 +88,5 @@ except (OSError, subprocess.CalledProcessError):
     card = torch.cuda.get_device_name() + " (power limit not readable)"
 print(json.dumps({"card": card, "boards": s.n_boards, "spec_s": t_spec, "build_s": t_build, "ms_per_iteration": it_ms,
                   "iterations_per_s": 1e3 / it_ms, "update_sweep_forms": res, "eval_both_ms": eval_ms, "expl_cur": a,
-                  "expl_avg": b, "mem_GB": torch.cuda.max_memory_allocated() / 2 ** 30, "grid": s.g.grid}))
+                  "expl_avg": b, "mem_GB": torch.cuda.max_memory_allocated() / 2 ** 30, "grid": s.g.grid,
+                  **({"stack": stack, "rows_per_board": s.rows_per_board} if stack != 20000 else {})}))

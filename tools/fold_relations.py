@@ -1,11 +1,13 @@
-"""Derives the table `FoldLinFHP` of csrc/cfr_board.cu: for the compiled post-deal shape of Flop5Holdem, the opponent's reach at
+"""Derives the tables `fold_coef` of csrc/cfr_board.cu: for a compiled post-deal shape of Flop5Holdem, the opponent's reach at
 every FOLD terminal as a +-1 combination of its reach at the SHOWDOWN terminals (the opponent's strategies sum to one at its
 own nodes, the sweep's seat copies the reach at its nodes).  The sweep kernel uses it to get the card-row sums of the fold
 vectors from the showdown vectors' row totals instead of gathering them (update form).
 
-    python tools/fold_relations.py        # prints the table in the C initialiser's layout
+    python tools/fold_relations.py        # prints the table of ShapeFHP in the C initialiser's layout
+    python tools/fold_relations.py 1,0,0,4,1,3,4,3,4 1,3,5,-1,7,-1,-1,-1,-1 2,2,2,0,2,0,0,0,0
+                                          # ... of the shape with these kind / first_child / n_children arrays (ShapeFHPShort)
 
-Method: random strategies -> reach of the opponent at all 15 nodes -> least squares of each fold vector on the five showdown
+Method: random strategies -> reach of the opponent at every node -> least squares of each fold vector on the showdown
 vectors; the residual must vanish and the coefficients must be integers."""
 import numpy as np
 
@@ -50,4 +52,8 @@ def as_c_initialiser(tab):
 
 
 if __name__ == "__main__":
-    print(as_c_initialiser(derive()))
+    import sys
+    if len(sys.argv) == 4:
+        print(as_c_initialiser(derive(*([int(x) for x in a.split(",")] for a in sys.argv[1:]))))
+    else:
+        print(as_c_initialiser(derive()))
