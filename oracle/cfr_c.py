@@ -29,6 +29,8 @@ def lib():
         L.orc_value_pass.argtypes = [tp, bp, C.c_int, C.c_int, ip]
         L.orc_root_exploitability.argtypes = [tp, bp, C.c_void_p]
         L.orc_cfr_half_iteration.argtypes = [tp, bp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, ip]
+        L.orc_pairwise_sum.argtypes = [C.c_void_p, C.c_int]
+        L.orc_pairwise_sum.restype = C.c_float
         _lib = L
     return _lib
 

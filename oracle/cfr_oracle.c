@@ -62,6 +62,32 @@ static double strat_f64(const ctx_t* c, int m, int slot, int fs, int A, int h) {
     return (double)(tab[(size_t)slot * ld + h] / s);
 }
 
+/* np.sum's order over a contiguous float32 row of n >= 1 elements: numpy's pairwise_sum (loops_utils.h.src), restated
+ * in oracle/pairwise_sum.py.  Fewer than 8 elements in order; up to 128, 8 interleaved partial sums combined as
+ * ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)), then the last n % 8 elements in order; above 128, the two halves split at
+ * n/2 rounded down to a multiple of 8.  np.sum adds the total to +0.0, which only changes the sign of a -0.0 total;
+ * that add is left out, as in the kernels. */
+float orc_pairwise_sum(const float* a, int n) {
+    if (n < 8) {
+        float s = a[0];
+        for (int i = 1; i < n; ++i) s = s + a[i];
+        return s;
+    }
+    if (n <= 128) {
+        float r[8];
+        for (int j = 0; j < 8; ++j) r[j] = a[j];
+        int i = 8;
+        for (; i < n - n % 8; i += 8)
+            for (int j = 0; j < 8; ++j) r[j] = r[j] + a[i + j];
+        float s = ((r[0] + r[1]) + (r[2] + r[3])) + ((r[4] + r[5]) + (r[6] + r[7]));
+        for (; i < n; ++i) s = s + a[i];
+        return s;
+    }
+    int n2 = n / 2;
+    n2 -= n2 % 8;
+    return orc_pairwise_sum(a, n2) + orc_pairwise_sum(a + n2, n - n2);
+}
+
 static int leduc_rank(const prl_tree_t* T, int h, int b) { /* game_rules.py:68-75 */
     int r = h / T->n_suits;
     return (b / T->n_suits == r) ? T->pair_bonus + r : r;
@@ -150,10 +176,8 @@ static float terminal_equity(const ctx_t* c, int n, int h, int p, int kind) {
     const float K = (float)((double)T->n_deck / (double)(T->n_deck - 1)); /* ValueFiller.py:19 */
     const int b = T->board[n];
     float eq;
-    if (kind == PRL_KIND_FOLD) { /* ValueFiller.py:103-125 */
-        float s = ro[0];
-        for (int j = 1; j < R; ++j) s = s + ro[j];
-        eq = s - ro[h];
+    if (kind == PRL_KIND_FOLD) { /* ValueFiller.py:103-125 (np.sum over the opponent's hands) */
+        eq = orc_pairwise_sum(ro, R) - ro[h];
         if (T->acted_last[n] == p) eq = -eq;
         eq = eq * K;
     } else if (kind == PRL_KIND_SHOWDOWN) { /* ValueFiller.py:127-158 */
@@ -272,12 +296,9 @@ int orc_root_exploitability(const prl_tree_t* T, const prl_buffers_t* B, float* 
         const float* ev = B->ev + (size_t)p * N * T->ld;
         const float* evbr = B->ev_br + (size_t)p * N * T->ld;
         const float* reach = B->reach + (size_t)p * N * T->ld;
-        float s = 0.0f;
-        for (int h = 0; h < T->n_range; ++h) {
-            const float e = evbr[h] * reach[h] - ev[h] * reach[h];
-            s = (h == 0) ? e : s + e;
-        }
-        out[p] = s;
+        float e[T->n_range];
+        for (int h = 0; h < T->n_range; ++h) e[h] = evbr[h] * reach[h] - ev[h] * reach[h];
+        out[p] = orc_pairwise_sum(e, T->n_range); /* np.sum(node.epsilon, axis=1) */
     }
     return 0;
 }

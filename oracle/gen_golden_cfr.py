@@ -10,6 +10,13 @@ What is pinned (all arrays DFS pre-order, see oracle/ref_harness.py):
                        profile (StrategyFiller.py:48-86, 118-146; ValueFiller.py:21-175)
   cfr_<algo>_<game>.npz  exploitability series logged by _CFRBase.py:198-262 and full regret / strategy /
                        average-strategy snapshots at selected iterations (CFRPlus.py, LinearCFR.py, VanillaCFR.py)
+
+BigLeduc (12 207 nodes, 24 hands) stores SHA-256 digests of its per-node arrays instead (oracle/fixture_digest.py,
+keys ending in "_sha256"), plus the root rows and the series in full.  Its second value profile is not the seeded
+random one but `fixture_digest.formula_strategy`, which the tests rebuild.  The reference's BigLeduc hand rank is run
+with the one NumPy 2 fix of ref_harness._patch_big_leduc_hand_rank.
+
+    python oracle/gen_golden_cfr.py BigLeduc   # only the fixtures of the named games
 """
 import hashlib
 import os
@@ -21,6 +28,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import ref_harness as rh  # noqa: E402
+from fixture_digest import array_digest, formula_strategy  # noqa: E402
 
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
 
@@ -30,7 +38,18 @@ GAMES = {
     "NLLeduc_POT": ("DiscretizedNLLeduc", "POT_ONLY"),
     "NLLeduc_B2": ("DiscretizedNLLeduc", "B_2"),
     "NLLeduc_B3": ("DiscretizedNLLeduc", "B_3"),
+    "BigLeduc": ("BigLeduc", "POT_ONLY"),
 }
+DIGEST_GAMES = ("BigLeduc",)  # per-node arrays stored as digests
+
+
+def fill_formula_profile(tree):
+    """Decision-node strategies of fixture_digest.formula_strategy (chance nodes keep the uniform fill's), reach."""
+    tree.fill_uniform_random()
+    for i, n in enumerate(rh.dfs_nodes(tree)):
+        if not n.is_terminal and n.p_id_acting_next in (0, 1):
+            n.strategy = formula_strategy(i, len(n.children), tree.env_bldr.rules.RANGE_SIZE)
+    tree.update_reach_probs()
 
 
 def _make_tree(game):
@@ -73,7 +92,21 @@ def gen_tree(game):
     out["uniform_root_ev"] = tree.root.ev
     out["uniform_root_ev_br"] = tree.root.ev_br
     out["uniform_root_exploitability"] = tree.root.exploitability
-    if len(s["parent"]) < 5000:
+    out["uniform_root_reach"] = tree.root.reach_probs
+    out["numpy_version"] = np.array(np.__version__)
+    if game in DIGEST_GAMES:
+        for k, v in rh.flatten_values(tree, R).items():
+            if k != "strat":
+                out["uniform_%s_sha256" % k] = np.array(array_digest(v))
+        fill_formula_profile(tree)
+        tree.compute_ev()
+        for k, v in rh.flatten_values(tree, R).items():
+            out["formula_%s_sha256" % k] = np.array(array_digest(v))
+        out["formula_root_reach"] = tree.root.reach_probs
+        out["formula_root_ev"] = tree.root.ev
+        out["formula_root_ev_br"] = tree.root.ev_br
+        out["formula_root_exploitability"] = tree.root.exploitability
+    elif len(s["parent"]) < 5000:
         np.random.seed(1234)
         tree.fill_random_random()
         tree.compute_ev()
@@ -107,7 +140,20 @@ def gen_cfr(job):
     R = cfr._env_bldrs[0].rules.RANGE_SIZE
     out = {}
 
+    def snap_digests(t):
+        v = rh.flatten_values(tree, R)
+        arrs = dict(regret=rh.flatten_node_table(tree, "regret", R), strat=v["strat"],
+                    avg=rh.flatten_node_table(tree, "avg_strat", R), reach=v["reach"], ev=v["ev"], ev_br=v["ev_br"])
+        if algo != "CFRPlus":
+            arrs["avg_sum"] = rh.flatten_node_table(tree, "avg_strat_sum", R)
+        for k, a in arrs.items():
+            out["it%d_%s_sha256" % (t, k)] = np.array(array_digest(a))
+        out["it%d_root_ev" % t] = tree.root.ev
+        out["it%d_root_ev_br" % t] = tree.root.ev_br
+
     def snap(t):
+        if game in DIGEST_GAMES:
+            return snap_digests(t)
         v = rh.flatten_values(tree, R)
         reg = rh.flatten_node_table(tree, "regret", R)
         out["it%d_regret" % t] = reg
@@ -142,7 +188,9 @@ def gen_cfr(job):
 
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
+    only = sys.argv[1:] or list(GAMES)
     snaps = (0, 1, 2, 3, 4, 5, 10, 11, 30, 31)
+    big_snaps = (0, 1, 2, 3, 10, 31)
     cfr_jobs = [
         ("CFRPlus", "NLLeduc_POT", 150, snaps + (150,)),
         ("CFRPlus", "StandardLeduc", 60, snaps),
@@ -150,10 +198,14 @@ if __name__ == "__main__":
         ("LinearCFR", "StandardLeduc", 40, snaps),
         ("VanillaCFR", "NLLeduc_POT", 40, snaps),
         ("VanillaCFR", "StandardLeduc", 40, snaps),
+        ("CFRPlus", "BigLeduc", 60, big_snaps),
+        ("LinearCFR", "BigLeduc", 40, big_snaps),
+        ("VanillaCFR", "BigLeduc", 40, big_snaps),
     ]
+    cfr_jobs = [j for j in cfr_jobs if j[1] in only]
     with Pool(8) as pool:
         r1 = pool.map_async(gen_cfr, cfr_jobs)
-        r2 = pool.map_async(gen_tree, list(GAMES))
+        r2 = pool.map_async(gen_tree, [g for g in GAMES if g in only])
         for r in r2.get():
             print("tree", r)
         for r in r1.get():

@@ -1,6 +1,6 @@
 """Golden PokerEnv trajectories produced by RUNNING THE REFERENCE ENV (TEST INFRASTRUCTURE; needs a PokerRL checkout in POKERRL_REFERENCE):
 
-    python oracle/gen_golden_env.py        # writes tests/golden/env_<game>.npz
+    python oracle/gen_golden_env.py [game ...]   # writes tests/golden/env_<game>.npz (default: every game)
 
 For each game: E episodes of uniformly random legal play in evaluation mode (PokerEnv.py:1075-1159,
 DiscretizedPokerEnv.py:47-135, LimitPokerEnv.py:27-59).  Recorded per episode: the shuffled deck (1D card ids, top
@@ -24,6 +24,7 @@ GAMES = {
     "StandardLeduc": ("StandardLeduc", "POT_ONLY", 13, 200),
     "LimitHoldem": ("LimitHoldem", "POT_ONLY", 48, 300),
     "Flop5Holdem": ("Flop5Holdem", "POT_ONLY", 20000, 200),
+    "BigLeduc": ("BigLeduc", "POT_ONLY", 100, 200),  # pair bonus 10000: runs with ref_harness's hand-rank fix
 }
 T_MAX = 48
 
@@ -75,5 +76,5 @@ def run(name):
 
 
 if __name__ == "__main__":
-    for n in GAMES:
+    for n in sys.argv[1:] or GAMES:
         print(run(n))

@@ -29,7 +29,27 @@ def import_reference():
         if p not in sys.path:
             sys.path.insert(0, p)
     import PokerRL  # noqa
+    _patch_big_leduc_hand_rank()
     return PokerRL
+
+
+def _patch_big_leduc_hand_rank():
+    """The ONLY deviation from the reference's code: BigLeducRules.get_hand_rank (game_rules.py:133-140) computes
+    `10000 + hand_2d[0, 0]` on an int8 scalar, which raises OverflowError under NumPy 2 (NEP 50).  NumPy < 2 promoted
+    it to int16 and returned 10000 + rank; this evaluates the same expression on a Python int, which is that value."""
+    from PokerRL.game._.rl_env.game_rules import BigLeducRules
+
+    if getattr(BigLeducRules.get_hand_rank, "_python_int_pair_bonus", False):
+        return
+
+    def get_hand_rank(self, hand_2d, board_2d):
+        if board_2d[0, 0] == hand_2d[0, 0]:
+            return 10000 + int(hand_2d[0, 0])
+        else:
+            return hand_2d[0, 0]
+
+    get_hand_rank._python_int_pair_bonus = True
+    BigLeducRules.get_hand_rank = get_hand_rank
 
 
 # node kind codes shared with pokerrl_b200.game.flat_tree

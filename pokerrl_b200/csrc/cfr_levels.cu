@@ -11,8 +11,9 @@
 // parallelism and launch count - not tensor cores.
 //
 // Arithmetic contract: every expression is evaluated in the reference's dtype and operation order
-// (oracle/cfr_numpy.py and oracle/cfr_oracle.c are pinned bit-for-bit against the reference).  This translation unit
-// is compiled with -fmad=false so that no multiply-add is contracted; the reference (numpy) never fuses.
+// (oracle/cfr_numpy.py and oracle/cfr_oracle.c are pinned bit-for-bit against the reference); a sum over a row of hands
+// follows np.sum, which is pairwise from 8 elements on (numpy_sum).  This translation unit is compiled with
+// -fmad=false so that no multiply-add is contracted; the reference (numpy) never fuses.
 //
 // Reference statements restated here (paths under PokerRL/):
 //   reach pass      game/_/tree/_/StrategyFiller.py:118-146, 148-169
@@ -122,6 +123,37 @@ __device__ __forceinline__ double strat_f64(const Ctx& c, int m, int fs, int k, 
     for (int j = 1; j < A; ++j) tot = tot + tab[(size_t)(fs + j) * ld + h];
     if (tot == 0.0f) return 1.0 / (double)A;
     return (double)(tab[(size_t)(fs + k) * ld + h] / tot);
+}
+
+// float sum of x(0) .. x(n - 1) in numpy's order (np.sum of a float32 row: pairwise_sum in
+// numpy/_core/src/umath/loops_utils.h.src, restated in oracle/pairwise_sum.py), for 1 <= n <= 128 and n <= NMAX.
+// Fewer than 8 elements are added in order.  From 8 on, 8 interleaved partial sums r[j] = x(j) + x(j + 8) + ... run
+// over the first n - n % 8 elements and are combined as ((r0 + r1) + (r2 + r3)) + ((r4 + r5) + (r6 + r7)); the last
+// n % 8 elements follow in order.  numpy also adds the total to the identity +0.0, which only turns a total of -0.0
+// into +0.0; that add is left out.  With NMAX < 8 (Leduc's rows of 6) only the sequential loop is compiled.
+template <int NMAX, class F>
+__device__ __forceinline__ float numpy_sum(const int n, F x) {
+    if constexpr (NMAX >= 8) {
+        if (n >= 8) {
+            float r[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) r[j] = x(j);
+            int i = 8;
+            for (; i < n - n % 8; i += 8) {
+#pragma unroll
+                for (int j = 0; j < 8; ++j) r[j] = r[j] + x(i + j);
+            }
+            float s = ((r[0] + r[1]) + (r[2] + r[3])) + ((r[4] + r[5]) + (r[6] + r[7]));
+            for (; i < n; ++i) s = s + x(i);
+            return s;
+        }
+    }
+    float s = 0.0f;
+    for (int i = 0; i < n; ++i) {
+        const float e = x(i);
+        s = (i == 0) ? e : s + e;
+    }
+    return s;
 }
 
 // hand rank of card h on board card b (game_rules.py:68-75); NS = N_SUITS (compile time)
@@ -242,10 +274,8 @@ __device__ __forceinline__ float terminal_value(const Ctx& c, const Meta& m, int
     for (int j = 0; j < R; ++j) ro[j] = __shfl_sync(L.gmask, mine, L.base + j);
     const float K = (float)((double)c.T.n_deck / (double)(c.T.n_deck - 1));  // ValueFiller.py:19
     float eq;
-    if (m.kind == PRL_KIND_FOLD) {  // ValueFiller.py:103-125
-        float s = ro[0];
-#pragma unroll
-        for (int j = 1; j < R; ++j) s = s + ro[j];
+    if (m.kind == PRL_KIND_FOLD) {  // ValueFiller.py:103-125 (np.sum over the opponent's hands)
+        const float s = numpy_sum<R>(R, [&](int j) { return ro[j]; });
         eq = s - mine;
         if (m.acted_last == p) eq = -eq;
         eq = eq * K;
@@ -462,17 +492,15 @@ __device__ __forceinline__ void stamp(const Levels& lv, int& slot) {
     ++slot;
 }
 
+// root exploitability of seat p (ValueFiller.py:95-101): np.sum over hands of ev_br * reach - ev * reach; NMAX bounds
+// T.n_range (see numpy_sum)
+template <int NMAX>
 __device__ __forceinline__ void root_exploitability(const prl_tree_t& T, const prl_buffers_t& B, int p, float* out) {
     const size_t N = (size_t)T.n_nodes;
     const float* ev = B.ev + (size_t)p * N * T.ld;
     const float* evbr = B.ev_br + (size_t)p * N * T.ld;
     const float* reach = B.reach + (size_t)p * N * T.ld;
-    float s = 0.0f;
-    for (int h = 0; h < T.n_range; ++h) {
-        const float e = evbr[h] * reach[h] - ev[h] * reach[h];
-        s = (h == 0) ? e : s + e;
-    }
-    out[p] = s;
+    out[p] = numpy_sum<NMAX>(T.n_range, [&](int h) { return evbr[h] * reach[h] - ev[h] * reach[h]; });
 }
 
 // THREADS: block size = threads per SM (one block per SM): 512 at 128 registers per thread.  A 1024-thread / 64-register
@@ -531,23 +559,14 @@ __global__ void __launch_bounds__(kPThreads, 1) evaluate_kernel(Ctx c, const Lev
         for (int grp = gwarp; grp < ng; grp += nwarps) value_group<R, NS, true, false>(c, lo, hi, grp);
         grid.sync();
     }
-    if (blockIdx.x == 0 && threadIdx.x < 2) root_exploitability(c.T, c.B, threadIdx.x, out);
+    if (blockIdx.x == 0 && threadIdx.x < 2) root_exploitability<R>(c.T, c.B, threadIdx.x, out);
 }
 
-// root exploitability (ValueFiller.py:95-101): sequential float sums like numpy's short contiguous reduction
+// root exploitability (ValueFiller.py:95-101) of both seats, one thread each; ranges of up to 128 hands
 __global__ void root_exploitability_kernel(prl_tree_t T, prl_buffers_t B, float* out) {
     const int p = threadIdx.x;
     if (p >= 2) return;
-    const size_t N = (size_t)T.n_nodes;
-    const float* ev = B.ev + (size_t)p * N * T.ld;
-    const float* evbr = B.ev_br + (size_t)p * N * T.ld;
-    const float* reach = B.reach + (size_t)p * N * T.ld;
-    float s = 0.0f;
-    for (int h = 0; h < T.n_range; ++h) {
-        const float e = evbr[h] * reach[h] - ev[h] * reach[h];
-        s = (h == 0) ? e : s + e;
-    }
-    out[p] = s;
+    root_exploitability<128>(T, B, p, out);
 }
 
 // one warp per group of `npw` nodes

@@ -14,6 +14,7 @@ GAMES = {
     "NLLeduc_POT": ("DiscretizedNLLeduc", "POT_ONLY"),
     "NLLeduc_B2": ("DiscretizedNLLeduc", "B_2"),
     "NLLeduc_B3": ("DiscretizedNLLeduc", "B_3"),
+    "BigLeduc": ("BigLeduc", "POT_ONLY"),
 }
 
 
@@ -27,3 +28,14 @@ def make_flat_tree(name):
 
 def golden(fname):
     return np.load(os.path.join(GOLDEN, fname), allow_pickle=False)
+
+
+def formula_profile_table(ft):
+    """oracle/fixture_digest.formula_strategy of every decision node (the second value profile of the BigLeduc
+    fixtures) as a float64 [n_slots, R] strategy table: row slot[c] = probability of moving to child c, per hand."""
+    from fixture_digest import formula_strategy
+    tab = np.zeros((ft.n_slots, ft.R))
+    for n in np.nonzero((ft.kind <= 1) & (ft.first_child >= 0))[0]:
+        A, fs = int(ft.n_children[n]), int(ft.first_slot[n])
+        tab[fs:fs + A] = formula_strategy(int(ft.dfs[n]), A, ft.R).T
+    return tab

@@ -9,7 +9,7 @@ from pokerrl_b200.game import bet_sets, games
 from pokerrl_b200.game import hu_engine as eng
 
 GAMES = ["DiscretizedNLHoldem_B5", "DiscretizedNLHoldem_B5_short", "DiscretizedNLLeduc_B3", "StandardLeduc", "LimitHoldem",
-         "Flop5Holdem"]
+         "Flop5Holdem", "BigLeduc"]
 
 
 @pytest.mark.parametrize("name", GAMES)
