@@ -98,6 +98,11 @@ def build_board_blobs(rules, boards, t_blob, dev):
                  C.c_void_p(t_hc.data_ptr()), n, C.c_void_p(t_blob[i:i + n].data_ptr()), _stream(dev))
 
 
+def _decision_locals(st):
+    """post-deal decision nodes, ascending local id (the columns of prl_board_policy_query's out_index)"""
+    return [i for i in range(st["n_local"]) if st["kind"][i] <= 1 and st["n_children"][i] > 0]
+
+
 def board_game(st, rules, n_boards, ld, n_sym, grid=0):
     """prl_board_game_t of a post-deal subtree `st` over n_boards boards, without buffers: shape, eq_const, the fixed-point
     format of the chance sums (which depends on n_sym, not on the boards) and the board-major row layout.
@@ -111,7 +116,7 @@ def board_game(st, rules, n_boards, ld, n_sym, grid=0):
     bound = max(n_sym, 1) * g.eq_const * max(st["pot"]) * 0.5 * 4.0
     g.frac_bits = 62 - int(math.ceil(math.log2(bound)))
     n_local = st["n_local"]
-    dec = [i for i in range(n_local) if st["kind"][i] <= 1]
+    dec = _decision_locals(st)
     rows_per_board = sum(st["n_children"][i] for i in dec)
     # board-major rows: everything a (board, seat) unit touches is contiguous - row(i, j) = j * rows_per_board + row_of[i]
     row_of, rpb = shape_rows(g)
@@ -128,11 +133,40 @@ def board_game(st, rules, n_boards, ld, n_sym, grid=0):
     return g, rows_per_board, local_rows
 
 
-class _BoardTrunk:
-    """The pre-deal trunk shared by the solver and the policy evaluator: a one-board flat tree carries the trunk and the
-    shape of the post-deal subtree; the trunk is swept by prl_board_trunk / the level kernels over its own small buffers."""
+def row_map(local_rows, ft=None):
+    """(src, dst), the prl_board_permute descriptors: for every row of the post-deal decision nodes, {row on board 0, stride
+    per board} in the strength-ordered table (src) and in the natural table (dst) - the slot table of the flat tree `ft` over
+    a chunk of boards, or without `ft` [boards, rows] with each board's rows in ascending local node order"""
+    st = None if ft is None else ft.board_subtree()
+    src, dst = [], []
+    for k, (i, (r0, m)) in enumerate(sorted(local_rows.items())):
+        src += [r0, m]
+        dst += [k, len(local_rows)] if ft is None else [int(ft.slot[st["node_base"][i] + st["node_k"][i]]), st["node_m"][i]]
+    return src, dst
 
-    def _init_trunk(self, game_cls, env_args, dev):
+
+def _normalised(x, dim, matching):
+    """x divided by its sums along `dim` (the actions), uniform where there is nothing to divide: regret matching
+    (matching: x clamped at 0, sums > 0) or normalised reach-weighted sums (sums != 0)"""
+    if matching:
+        x = x.clamp(min=0)
+    tot = x.sum(dim=dim, keepdim=True)
+    ok = (tot > 0) if matching else (tot != 0)
+    return torch.where(ok, x / torch.where(ok, tot, torch.ones_like(tot)), torch.full_like(x, 1.0 / x.shape[dim]))
+
+
+class _BoardEngine:
+    """What the solver and the policy evaluator share: the pre-deal trunk, swept by prl_board_trunk / the level kernels over
+    its own small buffers, the descriptor `g` of the post-deal subtrees of the boards, and the one call site of each board
+    entry point.  A one-board flat tree carries the trunk and the shape of the post-deal subtree."""
+
+    def _setup(self, game_cls, env_args, spec, n_boards, grid=0):
+        """the one-board trunk tree, the suit-symmetry tables of `spec`, the descriptor `g` over n_boards boards with the
+        buffers both engines bind, and the size of the game's tree over all the boards of `spec`"""
+        dev = self.device
+        self.rules = game_cls.RULES
+        self.ev_normalizer = game_cls.EV_NORMALIZER
+        self.L = board_layout()
         self.ft1 = FlatTree(game_cls, env_args, board_spec=_one_board_spec())
         st = self.ft1.board_subtree()
         if st is None:
@@ -140,7 +174,7 @@ class _BoardTrunk:
         self.st = st
         self.chance_level = st["chance_level"]
         self.chance_node = st["chance_node"]
-        self.R = game_cls.RULES.RANGE_SIZE
+        self.R = self.rules.RANGE_SIZE
         # trunk: level sweeps over levels 0 .. chance_level of the one-board tree; the symmetrisation over the suit
         # permutations happens in prl_board_collect / prl_board_trunk (integer sums), not in the level kernels
         self.trunk = DeviceTree(self.ft1, dev)
@@ -148,6 +182,36 @@ class _BoardTrunk:
         self.trunk.desc.sym_perm = None
         self.bufs = TreeBuffers(self.trunk)
         self.ld = self.trunk.ld
+        sp = spec.sym_perm
+        self.n_sym = 0 if sp is None else int(sp.shape[0])
+        self.t_sym = None if sp is None else torch.from_numpy(np.ascontiguousarray(sp, np.int16)).to(dev)
+        g, self.rows_per_board, self.local_rows = board_game(st, self.rules, n_boards, self.ld, self.n_sym, grid)
+        self.w_private = torch.zeros((g.grid, 2, self.R), dtype=torch.int64, device=dev)
+        self._expl = torch.zeros(2, dtype=torch.float32, device=dev)
+        g.w_private = self.w_private.data_ptr()
+        self.g = g
+        nb = self.n_boards_total = int(spec.boards.shape[0])
+        self.n_nodes = int(self.ft1.level_start[self.chance_level + 1]) + nb * st["n_local"]
+        self.n_nonterm = (int((self.ft1.kind[:self.chance_node + 1] <= nat.KIND_CHANCE).sum())
+                          + nb * len(_decision_locals(st)))
+
+    def _setup_boards(self, capacity):
+        """the per-board tables, probabilities and multiplicities for `capacity` boards (at least one), bound to `g`"""
+        dev, n = self.device, max(capacity, 1)
+        self.t_blob = torch.empty((n, self.L["blob"]), dtype=torch.uint8, device=dev)
+        self.t_prob = torch.zeros(n, dtype=torch.float32, device=dev)
+        self.t_mult = torch.zeros(n, dtype=torch.float32, device=dev)
+        g = self.g
+        g.tables, g.board_prob, g.board_mult = self.t_blob.data_ptr(), self.t_prob.data_ptr(), self.t_mult.data_ptr()
+
+    def _load_boards(self, boards, prob, mult):
+        """`boards` with their probabilities and multiplicities into the first rows of t_blob / t_prob / t_mult, and `g`
+        over them"""
+        n = boards.shape[0]
+        build_board_blobs(self.rules, boards, self.t_blob, self.device)
+        self.t_prob[:n].copy_(torch.from_numpy(np.ascontiguousarray(prob, np.float32)))
+        self.t_mult[:n].copy_(torch.from_numpy(np.ascontiguousarray(mult, np.float32)))
+        self.g.n_boards = n
 
     def _trunk_desc(self, bufs, modes):
         ft, t = self.ft1, nat.PrlTrunk()
@@ -168,17 +232,43 @@ class _BoardTrunk:
     def _trunk_reach_row(self, bufs, seat):
         return C.c_void_p(bufs.reach.data_ptr() + 4 * (seat * self.trunk.n_nodes + self.chance_node) * self.ld)
 
-    def _reach_trunk(self, bufs, mask, algo, upd_p, modes):
-        nat.call("prl_reach_levels", C.byref(self.trunk.desc), C.byref(bufs.desc), mask, algo, upd_p, self.iter_counter,
-                 self.delay, nat.modes(*modes), 0, self.chance_level, _stream(self.device))
+    def _reach_trunk(self, bufs, mask, algo, upd_p, modes, t, delay):
+        nat.call("prl_reach_levels", C.byref(self.trunk.desc), C.byref(bufs.desc), mask, algo, upd_p, t, delay,
+                 nat.modes(*modes), 0, self.chance_level, _stream(self.device))
 
     @property
     def n_trunk_slots(self):
         """table rows of the trunk: the first slots of every flat tree of the game (its children come before the deal)"""
-        return self.ft1.n_slots - sum(self.st["n_children"][i] for i in range(self.st["n_local"]) if self.st["kind"][i] <= 1)
+        return self.ft1.n_slots - self.rows_per_board
+
+    # ------------------------------------------------------------------------------------------------ board entry points
+    def _board_sweep(self, bufs, p, evaluate, src_own, src_opp, t, delay, algo, defer_w=0.0, p1_only=0):
+        """prl_board_sweep: seat p's update or evaluation sweep of the boards, against the opponent's trunk reach in `bufs`;
+        p1_only: the Vanilla / Linear CFR flush of the opponent's pending average contribution of weight defer_w"""
+        nat.call("prl_board_sweep", C.byref(self.g), p, int(evaluate), src_own, src_opp, self._trunk_reach_row(bufs, 1 - p),
+                 t, delay, algo, defer_w, p1_only, _stream(self.device))
+
+    def _board_trunk(self, bufs, modes, evaluate, p, t, delay, algo, peers=None, n_peers=0, peer_off=0, w_scratch=None):
+        """prl_board_trunk: the trunk of seat p's half-iteration, or of an evaluation of both seats into _expl, from the
+        chance sums `g` points at (peers: every rank's, summed in the kernel)"""
+        nat.call("prl_board_trunk", C.byref(self.g), C.byref(self._trunk_desc(bufs, modes)), int(evaluate), p, self.n_sym,
+                 C.c_void_p(self.t_sym.data_ptr()) if self.n_sym else None, t, delay, C.c_void_p(self._expl.data_ptr()), peers,
+                 n_peers, peer_off, w_scratch, algo, _stream(self.device))
+
+    def _board_permute(self, tab, nat_tab, to_natural, ft=None, lo=0, hi=None):
+        """prl_board_permute: the post-deal rows of boards lo .. hi (default: the boards `g` covers) from the strength-ordered
+        table `tab` to the natural table `nat_tab` (to_natural 1) or back (0); nat_tab's layout is that of row_map(ft)"""
+        g = self.g
+        if hi is not None:
+            g = nat.PrlBoardGame.from_buffer_copy(self.g)
+            g.n_boards, g.tables = hi - lo, self.t_blob[lo].data_ptr()
+        src, dst = (torch.tensor(x, dtype=torch.int64, device=self.device) for x in row_map(self.local_rows, ft))
+        nat.call("prl_board_permute", C.byref(g), len(self.local_rows), C.c_void_p(src.data_ptr()), C.c_void_p(dst.data_ptr()),
+                 C.c_void_p(tab[lo * self.rows_per_board].data_ptr()), C.c_void_p(nat_tab.data_ptr()), self.ld, to_natural,
+                 _stream(self.device))
 
 
-class BoardCFRSolver(_BoardTrunk):
+class BoardCFRSolver(_BoardEngine):
     def __init__(self, game_cls, env_args, board_spec=None, algo="CFRPlus", delay=0, device=None, rank=0, world=1,
                  group=None, grid=0, reduce_fn=None):
         if algo not in ALGOS:
@@ -189,54 +279,32 @@ class BoardCFRSolver(_BoardTrunk):
         self._reduce_fn = reduce_fn
         self.algo_name, self.algo = algo, ALGOS[algo]
         self.delay = int(delay) if algo == "CFRPlus" else 0
-        # Vanilla / Linear CFR: weight of the average-strategy contribution of each seat's last update that the post-deal rows
-        # have not received yet (it is added by the next sweep that walks those rows: csrc/cfr_board.cu, DEFER)
-        self._pending = [0.0, 0.0]
-        # CFR+: iteration of each seat's averaging step that is still pending (-1: none).  An update sweep with nothing pending
-        # leaves its step pending; the seat's next update sweep applies it together with its own (csrc/cfr_board.cu, AVG):
-        # every other sweep of a seat neither reads nor writes the average rows
-        self._avg_due = [-1, -1]
         self.game_cls, self.env_args = game_cls, env_args
-        rules = game_cls.RULES
-        spec = board_spec if board_spec is not None else BoardSpec.full_game(rules)
+        spec = board_spec if board_spec is not None else BoardSpec.full_game(game_cls.RULES)
         self.spec_full = spec
-        self.L = board_layout()
         with torch.cuda.device(self.device):
-            self._build(rules, spec, grid)
-        self.ev_normalizer = game_cls.EV_NORMALIZER
+            self._build(spec, grid)
         self.n_allreduce = 0
         self.reset()
 
     # ------------------------------------------------------------------------------------------------ construction
-    def _build(self, rules, spec, grid):
-        dev, L = self.device, self.L
-        self._init_trunk(self.game_cls, self.env_args, dev)
-        st = self.st
+    def _build(self, spec, grid):
+        dev = self.device
         sel = np.arange(self.rank, spec.boards.shape[0], self.world)
         self.board_ids = sel
         self.boards = np.ascontiguousarray(spec.boards[sel], np.int8)
         nb = self.n_boards = int(sel.size)
-        self.n_boards_total = int(spec.boards.shape[0])
+        self._setup(self.game_cls, self.env_args, spec, nb, grid)
         self.ops = TreeOps(self.trunk, self.bufs)
         self._eval_bufs = None
-        sp = spec.sym_perm
-        self.t_sym = None if sp is None else torch.from_numpy(np.ascontiguousarray(sp, np.int16)).to(dev)
-        self.n_sym = 0 if sp is None else int(sp.shape[0])
-        # per-board tables
-        self.t_blob = torch.empty((max(nb, 1), L["blob"]), dtype=torch.uint8, device=dev)
-        build_board_blobs(rules, self.boards, self.t_blob, dev)
+        self._setup_boards(nb)
+        self._load_boards(self.boards, spec.board_prob[sel], spec.board_mult[sel])
         torch.cuda.synchronize(dev)
-        self.t_prob = torch.from_numpy(np.ascontiguousarray(spec.board_prob[sel], np.float32)).to(dev)
-        self.t_mult = torch.from_numpy(np.ascontiguousarray(spec.board_mult[sel], np.float32)).to(dev)
-        n_local = st["n_local"]
-        dec = [i for i in range(n_local) if st["kind"][i] <= 1]
-        g, self.rows_per_board, self.local_rows = board_game(st, rules, nb, self.ld, self.n_sym, grid)
+        g = self.g
         self.n_rows = nb * self.rows_per_board
-        self.regret = torch.zeros((max(self.n_rows, 1), L["ldb"]), dtype=torch.float32, device=dev)
+        self.regret = torch.zeros((max(self.n_rows, 1), self.L["ldb"]), dtype=torch.float32, device=dev)
         self.avg = torch.zeros_like(self.regret)
-        g.tables, g.board_prob, g.board_mult = self.t_blob.data_ptr(), self.t_prob.data_ptr(), self.t_mult.data_ptr()
         g.regret, g.avg = self.regret.data_ptr(), self.avg.data_ptr()
-        self.w_private = torch.zeros((g.grid, 2, self.R), dtype=torch.int64, device=dev)
         # chance sums: two generations of [4][R] int64 (a sweep writes one generation while slow peers may still read the other)
         self._symm = None
         self.collective = "none" if self.world == 1 else "nccl all_reduce(int64)"
@@ -258,27 +326,36 @@ class BoardCFRSolver(_BoardTrunk):
         self._gen = 0
         self.w_total = self.w_gens[0]
         self.w_scratch = torch.zeros((4, self.R), dtype=torch.int64, device=dev)
-        g.w_private, g.w_total = self.w_private.data_ptr(), self.w_total.data_ptr()
-        self.g = g
+        g.w_total = self.w_total.data_ptr()
         # the trunk in one launch (prl_board_trunk); PRL_TRUNK=levels keeps the level-kernel chain (A/B, cross-check)
         self.fused_trunk = os.environ.get("PRL_TRUNK", "fused") != "levels"
-        self._expl = torch.zeros(2, dtype=torch.float32, device=dev)
         # where the level kernels expect the chance node's sums: prl_value_levels(chance_phase 1 / 2), one chance node,
         # one chunk -> W[arr] at float offset (4 + arr) * ld of the workspace
         self._w_off = 4 * self.ld
-        self.n_nodes = int(self.ft1.level_start[self.chance_level + 1]) + self.n_boards_total * n_local
-        self.n_nonterm = (int(((self.ft1.kind[:self.chance_node + 1] <= nat.KIND_CHANCE)).sum())
-                          + self.n_boards_total * len(dec))
 
     # ------------------------------------------------------------------------------------------------ helpers
+    def _clear_pending(self):
+        """no average-strategy update pending on either seat.
+        _pending (Vanilla / Linear CFR): weight of the average-strategy contribution of each seat's last update that the
+        post-deal rows have not received yet (it is added by the next sweep that walks those rows: csrc/cfr_board.cu, DEFER).
+        _avg_due (CFR+): iteration of each seat's averaging step that is still pending (-1: none).  An update sweep with
+        nothing pending leaves its step pending; the seat's next update sweep applies it together with its own
+        (csrc/cfr_board.cu, AVG): every other sweep of a seat neither reads nor writes the average rows."""
+        self._pending = [0.0, 0.0]
+        self._avg_due = [-1, -1]
+
     def _trunk(self, bufs, modes, evaluate, p):
         peers, n_peers, off = None, 0, 0
         if self._symm is not None:
             peers, n_peers, off = C.c_void_p(self._peer_ptrs.data_ptr()), self.world, self._gen * 4 * self.R
-        nat.call("prl_board_trunk", C.byref(self.g), C.byref(self._trunk_desc(bufs, modes)), int(evaluate), p, self.n_sym,
-                 C.c_void_p(self.t_sym.data_ptr()) if self.n_sym else None, self.iter_counter, self.delay,
-                 C.c_void_p(self._expl.data_ptr()), peers, n_peers, off, C.c_void_p(self.w_scratch.data_ptr()), self.algo,
-                 _stream(self.device))
+        self._board_trunk(bufs, modes, evaluate, p, self.iter_counter, self.delay, self.algo, peers, n_peers, off,
+                          C.c_void_p(self.w_scratch.data_ptr()))
+
+    def _board_update_cfrp(self, p, due, now):
+        """prl_board_update_cfrp: seat p's CFR+ update sweep of this iteration, writing its averaging step if `now` (else
+        leaving it pending) together with the pending step of iteration `due` (-1: none)"""
+        nat.call("prl_board_update_cfrp", C.byref(self.g), p, self._trunk_reach_row(self.bufs, 1 - p), self.iter_counter,
+                 self.delay, due, now, _stream(self.device))
 
     def _next_generation(self):
         """the next sweep(s) write the other generation of the chance sums"""
@@ -308,14 +385,12 @@ class BoardCFRSolver(_BoardTrunk):
             t, due = self.iter_counter, self._avg_due[p]
             now = 1 if due >= 0 or t < self.delay else 0  # an iteration before delay has no step to leave pending
             self._avg_due[p] = -1 if now else t
-            nat.call("prl_board_update_cfrp", C.byref(self.g), p, self._trunk_reach_row(bufs, 1 - p), t, self.delay, due, now,
-                     _stream(self.device))
+            self._board_update_cfrp(p, due, now)
             return
         defer_w = 0.0
         if not evaluate and self.algo != nat.ALGO_CFR_PLUS:  # this sweep walks the opponent's rows: its pending average goes in
             defer_w, self._pending[1 - p] = self._pending[1 - p], 0.0
-        nat.call("prl_board_sweep", C.byref(self.g), p, int(evaluate), src_own, src_opp, self._trunk_reach_row(bufs, 1 - p),
-                 self.iter_counter, self.delay, self.algo, defer_w, 0, _stream(self.device))
+        self._board_sweep(bufs, p, evaluate, src_own, src_opp, self.iter_counter, self.delay, self.algo, defer_w)
 
     def flush_average(self):
         """Applies the average-strategy updates that are still pending: CFR+ averaging steps (prl_board_avg_flush), Vanilla /
@@ -326,8 +401,8 @@ class BoardCFRSolver(_BoardTrunk):
                     nat.call("prl_board_avg_flush", C.byref(self.g), q, self._avg_due[q], self.delay, _stream(self.device))
                     self._avg_due[q] = -1
                 if self._pending[q] != 0.0:
-                    nat.call("prl_board_sweep", C.byref(self.g), 1 - q, 0, 0, 0, self._trunk_reach_row(self.bufs, q),
-                             self.iter_counter, self.delay, self.algo, self._pending[q], 1, _stream(self.device))
+                    self._board_sweep(self.bufs, 1 - q, False, 0, 0, self.iter_counter, self.delay, self.algo,
+                                      defer_w=self._pending[q], p1_only=1)
                     self._pending[q] = 0.0
 
     def _sweep_end(self, bufs, p, evaluate):
@@ -372,7 +447,7 @@ class BoardCFRSolver(_BoardTrunk):
         if cl > 0:
             self._levels(self.bufs, 1 << p, False, self.algo, p, self.modes, cl - 1, 0, 0)
         self.modes[p] = nat.STRAT_F32
-        self._reach_trunk(self.bufs, 1 << p, self.algo, p, self.modes)
+        self._reach_trunk(self.bufs, 1 << p, self.algo, p, self.modes, self.iter_counter, self.delay)
 
     # ------------------------------------------------------------------------------------------------ schedule
     def reset(self):
@@ -380,10 +455,9 @@ class BoardCFRSolver(_BoardTrunk):
             self.iter_counter = 0
             for t in (self.regret, self.avg, self.bufs.regret, self.bufs.strat, self.bufs.avg):
                 t.zero_()
-            self._pending = [0.0, 0.0]
-            self._avg_due = [-1, -1]
+            self._clear_pending()
             self.modes = [nat.STRAT_UNIFORM64, nat.STRAT_UNIFORM64]
-            self._reach_trunk(self.bufs, 3, -1, -1, self.modes)
+            self._reach_trunk(self.bufs, 3, -1, -1, self.modes, self.iter_counter, self.delay)
 
     def iteration(self, n=1):
         with torch.cuda.device(self.device):
@@ -430,7 +504,7 @@ class BoardCFRSolver(_BoardTrunk):
                 modes, src = [nat.STRAT_F32, nat.STRAT_F32], SRC_REGRET
             else:
                 modes, src = [nat.STRAT_AVG_F32, nat.STRAT_AVG_F32], SRC_AVG
-            self._reach_trunk(self._eval_bufs, 3, -1, -1, modes)
+            self._reach_trunk(self._eval_bufs, 3, -1, -1, modes, self.iter_counter, self.delay)
             return self._evaluate(self._eval_bufs, modes, src)
 
     # ------------------------------------------------------------------------------------------------ interfaces
@@ -439,65 +513,37 @@ class BoardCFRSolver(_BoardTrunk):
         THIS rank's boards (for agents, exports and parity tests on small instances)."""
         assert ft.board_spec.boards.shape[0] == self.n_boards
         self.flush_average()
-        st = ft.board_subtree()
-        out = []
-        dev = self.device
-        src, dst = [], []
-        for i, (r0, m) in sorted(self.local_rows.items()):
-            n0 = st["node_base"][i] + st["node_k"][i]
-            src += [r0, m]
-            dst += [int(ft.slot[n0]), st["node_m"][i]]
-        t_src = torch.tensor(src, dtype=torch.int64, device=dev)
-        t_dst = torch.tensor(dst, dtype=torch.int64, device=dev)
-        n_trunk_slots = self.bufs.regret.shape[0] - self.rows_per_board  # slots of the one-board trunk tree before the board
-        for tab, trunk_tab in ((self.regret, self.bufs.regret), (self.avg, self.bufs.avg)):
-            nat_tab = torch.zeros((ft.n_slots, self.ld), dtype=torch.float32, device=dev)
-            with torch.cuda.device(dev):
-                nat.call("prl_board_permute", C.byref(self.g), len(self.local_rows), C.c_void_p(t_src.data_ptr()),
-                         C.c_void_p(t_dst.data_ptr()), C.c_void_p(tab.data_ptr()), C.c_void_p(nat_tab.data_ptr()), self.ld, 1,
-                         _stream(dev))
-            nat_tab[:n_trunk_slots] = trunk_tab[:n_trunk_slots]
-            out.append(nat_tab)
+        nts, out = self.n_trunk_slots, []
+        with torch.cuda.device(self.device):
+            for tab, trunk_tab in ((self.regret, self.bufs.regret), (self.avg, self.bufs.avg)):
+                nat_tab = torch.zeros((ft.n_slots, self.ld), dtype=torch.float32, device=self.device)
+                self._board_permute(tab, nat_tab, 1, ft)
+                nat_tab[:nts] = trunk_tab[:nts]
+                out.append(nat_tab)
         return out
 
     def load_natural_tables(self, ft, regret, avg):
         """inverse of natural_tables (teacher forcing in the parity tests, checkpoints written by the level engine)"""
-        self._pending = [0.0, 0.0]  # the given average is complete
-        self._avg_due = [-1, -1]
-        st = ft.board_subtree()
-        dev = self.device
-        src, dst = [], []
-        for i, (r0, m) in sorted(self.local_rows.items()):
-            n0 = st["node_base"][i] + st["node_k"][i]
-            src += [r0, m]
-            dst += [int(ft.slot[n0]), st["node_m"][i]]
-        t_src = torch.tensor(src, dtype=torch.int64, device=dev)
-        t_dst = torch.tensor(dst, dtype=torch.int64, device=dev)
-        n_trunk_slots = self.bufs.regret.shape[0] - self.rows_per_board
-        for tab, trunk_tab, given in ((self.regret, self.bufs.regret, regret), (self.avg, self.bufs.avg, avg)):
-            nat_tab = torch.zeros((ft.n_slots, self.ld), dtype=torch.float32, device=dev)
-            nat_tab[:, :given.shape[1]] = torch.as_tensor(given, dtype=torch.float32).to(dev)
-            with torch.cuda.device(dev):
-                nat.call("prl_board_permute", C.byref(self.g), len(self.local_rows), C.c_void_p(t_src.data_ptr()),
-                         C.c_void_p(t_dst.data_ptr()), C.c_void_p(tab.data_ptr()), C.c_void_p(nat_tab.data_ptr()), self.ld, 0,
-                         _stream(dev))
-            trunk_tab[:n_trunk_slots] = nat_tab[:n_trunk_slots]
+        self._clear_pending()  # the given average is complete
+        nts, dev = self.n_trunk_slots, self.device
+        with torch.cuda.device(dev):
+            for tab, trunk_tab, given in ((self.regret, self.bufs.regret, regret), (self.avg, self.bufs.avg, avg)):
+                nat_tab = torch.zeros((ft.n_slots, self.ld), dtype=torch.float32, device=dev)
+                nat_tab[:, :given.shape[1]] = torch.as_tensor(given, dtype=torch.float32).to(dev)
+                self._board_permute(tab, nat_tab, 0, ft)
+                trunk_tab[:nts] = nat_tab[:nts]
 
     def set_trunk_strategy_from_regrets(self):
         """after load_natural_tables: the trunk's stored strategy rows = regret matching of its regret rows, reach rows
         refreshed (the post-deal rows need nothing: their strategy is never stored)"""
         ft = self.ft1
-        n_trunk_slots = self.bufs.regret.shape[0] - self.rows_per_board
-        r = torch.clamp(self.bufs.regret[:n_trunk_slots], min=0)
         for n in range(self.chance_node + 1):
             if ft.kind[n] <= 1 and ft.first_child[n] >= 0:
                 fs, A = int(ft.first_slot[n]), int(ft.n_children[n])
-                s = r[fs:fs + A].sum(dim=0, keepdim=True)
-                self.bufs.strat[fs:fs + A] = torch.where(s > 0, r[fs:fs + A] / torch.where(s > 0, s, torch.ones_like(s)),
-                                                         torch.full_like(s, 1.0 / A))
+                self.bufs.strat[fs:fs + A] = _normalised(self.bufs.regret[fs:fs + A], 0, True)
         self.modes = [nat.STRAT_F32, nat.STRAT_F32]
         with torch.cuda.device(self.device):
-            self._reach_trunk(self.bufs, 3, -1, -1, self.modes)
+            self._reach_trunk(self.bufs, 3, -1, -1, self.modes, self.iter_counter, self.delay)
 
     def state_dict(self):
         self.flush_average()
@@ -514,15 +560,14 @@ class BoardCFRSolver(_BoardTrunk):
         if tuple(state["regret"].shape) != tuple(self.regret.shape):
             raise ValueError("checkpoint table shape %s != %s" % (tuple(state["regret"].shape), tuple(self.regret.shape)))
         self.iter_counter, self.modes = int(state["iter_counter"]), list(state["modes"])
-        self._pending = [0.0, 0.0]  # state_dict() flushes before it exports
-        self._avg_due = [-1, -1]
+        self._clear_pending()  # state_dict() flushes before it exports
         self.regret.copy_(state["regret"])
         self.avg.copy_(state["avg"])
         self.bufs.regret.copy_(state["trunk_regret"])
         self.bufs.strat.copy_(state["trunk_strat"])
         self.bufs.avg.copy_(state["trunk_avg"])
         with torch.cuda.device(self.device):
-            self._reach_trunk(self.bufs, 3, -1, -1, self.modes)
+            self._reach_trunk(self.bufs, 3, -1, -1, self.modes, self.iter_counter, self.delay)
 
 
 # ==================================================================================================================== policy evaluation
@@ -535,21 +580,6 @@ def board_keys(boards):
     return key
 
 
-def _decision_locals(st):
-    """post-deal decision nodes, ascending local id (the columns of prl_board_policy_query's out_index)"""
-    return [i for i in range(st["n_local"]) if st["kind"][i] <= 1 and st["n_children"][i] > 0]
-
-
-def chunk_row_map(ft, st, local_rows):
-    """(src, dst): for every row of the post-deal decision nodes, {row on board 0, stride per board} in the strength-ordered
-    table and in the slot table of the flat tree `ft` over a chunk of boards (the prl_board_permute descriptors)"""
-    src, dst = [], []
-    for i, (r0, m) in sorted(local_rows.items()):
-        src += [r0, m]
-        dst += [int(ft.slot[st["node_base"][i] + st["node_k"][i]]), st["node_m"][i]]
-    return src, dst
-
-
 def abstract_fingerprint(ft):
     """identity of the betting structure of a flat tree (any board spec): kinds, actions, pots and fan-outs of its abstract
     nodes - equal for every spec of one game and stack"""
@@ -558,7 +588,7 @@ def abstract_fingerprint(ft):
     return hashlib.sha1(a.tobytes()).hexdigest()
 
 
-class BoardPolicyEvaluator(_BoardTrunk):
+class BoardPolicyEvaluator(_BoardEngine):
     """Exploitability of an agent's strategy on a game the board engine supports (single GPU), with the strategy supplied
     chunk by chunk over the boards of a BoardSpec, so that it never has to exist for the whole game at once.
 
@@ -590,46 +620,27 @@ class BoardPolicyEvaluator(_BoardTrunk):
         self.env_bldr, self.stack_size = env_bldr, stack_size
         game_cls = env_bldr.env_cls
         self.env_args = env_bldr.args_for_stack(stack_size)
-        rules = self.rules = game_cls.RULES
-        self.spec = board_spec if board_spec is not None else BoardSpec.full_game(rules)
-        self.iter_counter, self.delay = 0, 0
-        self.ev_normalizer = game_cls.EV_NORMALIZER
-        L = self.L = board_layout()
+        self.spec = board_spec if board_spec is not None else BoardSpec.full_game(game_cls.RULES)
         n_actions = env_bldr.N_ACTIONS
         with torch.cuda.device(dev):
-            self._init_trunk(game_cls, self.env_args, dev)
-            st = self.st
-            sp = self.spec.sym_perm
-            self.n_sym = 0 if sp is None else int(sp.shape[0])
-            self.t_sym = None if sp is None else torch.from_numpy(np.ascontiguousarray(sp, np.int16)).to(dev)
-            self.n_boards_total = nb = int(self.spec.boards.shape[0])
-            g, rpb, self.local_rows = board_game(st, rules, 0, self.ld, self.n_sym)
-            self.rows_per_board = rpb
-            n_dec = len(_decision_locals(st))
+            self._setup(game_cls, self.env_args, self.spec, 0)
+            L, rpb, g = self.L, self.rows_per_board, self.g
+            n_dec = len(_decision_locals(self.st))
             self.bytes_per_board = (L["blob"] + rpb * L["ldb"] * 4 + rpb * self.ld * 4 + n_dec * self.R * n_actions * 4
                                     + self.R * 4)
             if chunk is None:
                 free, _ = torch.cuda.mem_get_info(dev)
                 chunk = min(self.MAX_CHUNK, free // 2 // self.bytes_per_board)
-            self.chunk = max(1, min(int(chunk), nb))
+            self.chunk = max(1, min(int(chunk), self.n_boards_total))
             n = self.chunk
-            self.t_blob = torch.empty((n, L["blob"]), dtype=torch.uint8, device=dev)
+            self._setup_boards(n)
             self.rows = torch.zeros((n * rpb, L["ldb"]), dtype=torch.float32, device=dev)
             self.nat_tab = torch.zeros((self.n_trunk_slots + n * rpb, self.ld), dtype=torch.float32, device=dev)
-            self.t_prob = torch.zeros(n, dtype=torch.float32, device=dev)
-            self.t_mult = torch.zeros(n, dtype=torch.float32, device=dev)
-            self.w_private = torch.zeros((g.grid, 2, self.R), dtype=torch.int64, device=dev)
             self.w_total = torch.zeros((4, self.R), dtype=torch.int64, device=dev)
             self.w_acc = torch.zeros_like(self.w_total)
-            self._expl = torch.zeros(2, dtype=torch.float32, device=dev)
-            g.tables, g.board_prob, g.board_mult = self.t_blob.data_ptr(), self.t_prob.data_ptr(), self.t_mult.data_ptr()
             # evaluation with src 1 reads the strategy rows as they are and never the regrets: one table serves both
             g.regret = g.avg = self.rows.data_ptr()
-            g.w_private, g.w_total = self.w_private.data_ptr(), self.w_total.data_ptr()
-            self.g = g
-        self.n_nodes = int(self.ft1.level_start[self.chance_level + 1]) + nb * st["n_local"]
-        self.n_nonterm = (int((self.ft1.kind[:self.chance_node + 1] <= nat.KIND_CHANCE).sum())
-                          + nb * len([i for i in range(st["n_local"]) if st["kind"][i] <= 1]))
+            g.w_total = self.w_total.data_ptr()
         self.times = {}
 
     def _chunk_tree(self, lo, hi):
@@ -646,7 +657,7 @@ class BoardPolicyEvaluator(_BoardTrunk):
         """exploitability of each seat in chips, numpy float64 [2] (the analogue of PublicTree's root.exploitability).
         profile=True synchronises between the phases and leaves their wall times (s) in self.times."""
         import time
-        dev, g, R = self.device, self.g, self.R
+        dev, R, s = self.device, self.R, self.spec
         times = {"agent query": 0.0, "table build": 0.0, "sweeps": 0.0}
         modes = [nat.STRAT_AVG_F32, nat.STRAT_AVG_F32]
 
@@ -663,7 +674,6 @@ class BoardPolicyEvaluator(_BoardTrunk):
             nts = self.n_trunk_slots
             for lo in range(0, self.n_boards_total, self.chunk):
                 hi = min(lo + self.chunk, self.n_boards_total)
-                n = hi - lo
                 t0 = time.perf_counter()
                 pt = self._chunk_tree(lo, hi)
                 ft = pt.flat
@@ -672,31 +682,20 @@ class BoardPolicyEvaluator(_BoardTrunk):
                 if not isinstance(got, torch.Tensor):  # answered node by node on the host
                     tab[:, :R].copy_(torch.from_numpy(np.ascontiguousarray(got, np.float32)))
                 t0 = tick("agent query", t0)
-                build_board_blobs(self.rules, self.spec.boards[lo:hi], self.t_blob, dev)
-                self.t_prob[:n].copy_(torch.from_numpy(np.ascontiguousarray(self.spec.board_prob[lo:hi], np.float32)))
-                self.t_mult[:n].copy_(torch.from_numpy(np.ascontiguousarray(self.spec.board_mult[lo:hi], np.float32)))
-                g.n_boards = n
-                src, dst = chunk_row_map(ft, pt.flat.board_subtree(), self.local_rows)
-                t_src = torch.tensor(src, dtype=torch.int64, device=dev)
-                t_dst = torch.tensor(dst, dtype=torch.int64, device=dev)
-                nat.call("prl_board_permute", C.byref(g), len(self.local_rows), C.c_void_p(t_src.data_ptr()),
-                         C.c_void_p(t_dst.data_ptr()), C.c_void_p(self.rows.data_ptr()), C.c_void_p(tab.data_ptr()), self.ld, 0,
-                         _stream(dev))
+                self._load_boards(s.boards[lo:hi], s.board_prob[lo:hi], s.board_mult[lo:hi])
+                self._board_permute(self.rows, tab, 0, ft)
                 if lo == 0:  # the trunk's rows, then its reach: the sweeps read the opponent's reach at the chance node
                     self.bufs.avg[:nts].copy_(tab[:nts])
-                    self._reach_trunk(self.bufs, 3, -1, -1, modes)
+                    self._reach_trunk(self.bufs, 3, -1, -1, modes, 0, 0)
                 t0 = tick("table build", t0)
                 for p in (0, 1):  # prl_board_sweep zeroes the arrays it writes at every launch: accumulate outside
-                    nat.call("prl_board_sweep", C.byref(g), p, 1, SRC_AVG, SRC_AVG, self._trunk_reach_row(self.bufs, 1 - p), 0, 0,
-                             nat.ALGO_CFR_PLUS, 0.0, 0, _stream(dev))
+                    self._board_sweep(self.bufs, p, True, SRC_AVG, SRC_AVG, 0, 0, nat.ALGO_CFR_PLUS)
                     self.w_acc[2 * p:2 * p + 2] += self.w_total[2 * p:2 * p + 2]
                 tick("sweeps", t0)
                 del pt
             t0 = time.perf_counter()
             self.w_total.copy_(self.w_acc)
-            nat.call("prl_board_trunk", C.byref(g), C.byref(self._trunk_desc(self.bufs, modes)), 1, -1, self.n_sym,
-                     C.c_void_p(self.t_sym.data_ptr()) if self.n_sym else None, 0, 0, C.c_void_p(self._expl.data_ptr()), None, 0, 0,
-                     None, nat.ALGO_CFR_PLUS, _stream(dev))
+            self._board_trunk(self.bufs, modes, True, -1, 0, 0, nat.ALGO_CFR_PLUS)
             e = self._expl.cpu().numpy().astype(np.float64)
             tick("sweeps", t0)
         self.times = times
@@ -745,13 +744,7 @@ class BoardPolicyTables:
                 for lo in range(0, nb, 8192):
                     hi = min(lo + 8192, nb)
                     for idx in groups:
-                        x = src[lo:hi, idx]
-                        if matching:
-                            x = x.clamp(min=0)
-                        tot = x.sum(dim=1, keepdim=True)
-                        ok = (tot > 0) if matching else (tot != 0)
-                        dst[lo:hi, idx] = torch.where(ok, x / torch.where(ok, tot, torch.ones_like(tot)),
-                                                      torch.full_like(x, 1.0 / len(idx)))
+                        dst[lo:hi, idx] = _normalised(src[lo:hi, idx], 1, matching)
             nts, ft = s.n_trunk_slots, s.ft1
             if cfrp:
                 trunk = (s.bufs.strat if s.iter_counter == s.delay + 1 else s.bufs.avg)[:nts].clone()
@@ -761,9 +754,7 @@ class BoardPolicyTables:
                 for n in range(s.chance_node + 1):
                     if ft.kind[n] <= 1 and ft.first_child[n] >= 0:
                         fs, A = int(ft.first_slot[n]), int(ft.n_children[n])
-                        tot = a[fs:fs + A].sum(dim=0, keepdim=True)
-                        trunk[fs:fs + A] = torch.where(tot == 0, torch.full_like(a[fs:fs + A], 1.0 / A),
-                                                       a[fs:fs + A] / torch.where(tot == 0, torch.ones_like(tot), tot))
+                        trunk[fs:fs + A] = _normalised(a[fs:fs + A], 0, False)
             L = s.L
             pos_hand = s.t_blob[:nb, L["sh_off"]:L["sh_off"] + 2 * L["n_live"]].contiguous().view(torch.int16)
             keys = board_keys(s.boards)

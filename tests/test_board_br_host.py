@@ -37,13 +37,13 @@ def test_canonical_keys_reproduce_the_flop5_classes():
     assert np.array_equal(counts, orbit)
 
 
-def test_chunk_row_map_agrees_with_the_board_subtree():
+def test_row_map_agrees_with_the_board_subtree():
     """every post-deal slot of a chunk tree maps to row j * rows_per_board + row_of(local node) of its board j"""
-    from pokerrl_b200.board_engine import board_game, chunk_row_map
+    from pokerrl_b200.board_engine import board_game, row_map
     ft = fhp_tree(random_board_spec(23, 5))
     st = ft.board_subtree()
     _, rpb, local_rows = board_game(st, ft.rules, 23, 1328, 0, grid=1)
-    src, dst = chunk_row_map(ft, st, local_rows)
+    src, dst = row_map(local_rows, ft)
     got = {}
     for k in range(len(src) // 2):
         for j in range(23):

@@ -1,8 +1,6 @@
 """CFR+ averaging on the board engine two iterations at a time (csrc/cfr_board.cu, AVG; BoardCFRSolver._avg_due): an update
 sweep with nothing pending leaves its averaging step pending and the seat's next sweep applies both.  Every result must be the
 same bits as the immediate form, where each sweep writes its own step (prl_board_sweep), whatever interrupts the pairs."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -11,20 +9,20 @@ from twocard_common import random_board_spec
 pytestmark = pytest.mark.gpu
 
 
-def _engine(spec, immediate=False, **kw):
-    from pokerrl_b200 import _native as nat
-    from pokerrl_b200.board_engine import BoardCFRSolver, _stream
+def _engine(spec, immediate=False, args=None, **kw):
+    """Flop5Holdem with the game arguments `args` (default: stacks of 20 000 chips, pot-size bets)"""
+    from pokerrl_b200.board_engine import BoardCFRSolver
     from pokerrl_b200.game import games
 
     class Immediate(BoardCFRSolver):
         """every update sweep writes its own averaging step: the form before pairing, through the unchanged C entry point"""
 
         def _sweep_begin(self, bufs, p, evaluate, src_own, src_opp):
-            nat.call("prl_board_sweep", C.byref(self.g), p, int(evaluate), src_own, src_opp, self._trunk_reach_row(bufs, 1 - p),
-                     self.iter_counter, self.delay, self.algo, 0.0, 0, _stream(self.device))
+            self._board_sweep(bufs, p, evaluate, src_own, src_opp, self.iter_counter, self.delay, self.algo)
 
     g = games.Flop5Holdem
-    args = g.ARGS_CLS(n_seats=2, starting_stack_sizes_list=[20000, 20000], bet_sizes_list_as_frac_of_pot=[1.0])
+    if args is None:
+        args = g.ARGS_CLS(n_seats=2, starting_stack_sizes_list=[20000, 20000], bet_sizes_list_as_frac_of_pot=[1.0])
     return (Immediate if immediate else BoardCFRSolver)(g, args, spec, **kw)
 
 

@@ -48,38 +48,20 @@ class _Moves:
     """chunk-wise moves of post-deal rows between the engine's strength-ordered tables and [n, rows, R] natural tensors"""
 
     def __init__(self, e, rows):
-        import torch
-        assert [c for c, _ in sorted(e.local_rows.items())] == rows
-        src, dst = [], []
-        for k, (c, (r0, m)) in enumerate(sorted(e.local_rows.items())):
-            src += [r0, m]
-            dst += [k, len(rows)]
+        assert [c for c, _ in sorted(e.local_rows.items())] == rows  # the row order of board_engine.row_map without a tree
         self.e, self.n_rows = e, len(rows)
-        self.src = torch.tensor(src, dtype=torch.int64, device=e.device)
-        self.dst = torch.tensor(dst, dtype=torch.int64, device=e.device)
-
-    def _call(self, tab, lo, hi, nat_tab, to_natural):
-        import ctypes as C
-        from pokerrl_b200 import _native as nat
-        from pokerrl_b200.board_engine import _stream
-        e = self.e
-        g = nat.PrlBoardGame.from_buffer_copy(e.g)
-        g.n_boards, g.tables = hi - lo, e.t_blob[lo].data_ptr()
-        nat.call("prl_board_permute", C.byref(g), self.n_rows, C.c_void_p(self.src.data_ptr()), C.c_void_p(self.dst.data_ptr()),
-                 C.c_void_p(tab[lo * e.rows_per_board].data_ptr()), C.c_void_p(nat_tab.data_ptr()), e.ld, to_natural,
-                 _stream(e.device))
 
     def load(self, tab, lo, rows):
         import torch
         n = rows.shape[0]
         t = torch.zeros((n * self.n_rows, self.e.ld), dtype=torch.float32, device=self.e.device)
         t[:, :rows.shape[2]] = rows.reshape(n * self.n_rows, -1)
-        self._call(tab, lo, lo + n, t, 0)
+        self.e._board_permute(tab, t, 0, lo=lo, hi=lo + n)
 
     def fetch(self, tab, lo, hi):
         import torch
         t = torch.empty(((hi - lo) * self.n_rows, self.e.ld), dtype=torch.float32, device=self.e.device)
-        self._call(tab, lo, hi, t, 1)
+        self.e._board_permute(tab, t, 1, lo=lo, hi=hi)
         return t.view(hi - lo, self.n_rows, self.e.ld)[..., :self.e.R]
 
 
@@ -102,7 +84,7 @@ def _load(e, moves, prof, seat=0, due=-1):
     e.bufs.regret[:nts, :e.R], e.bufs.avg[:nts, :e.R] = tr, ta
     e.set_trunk_strategy_from_regrets()
     e.iter_counter = ITER
-    e._pending, e._avg_due = [0.0, 0.0], [-1, -1]
+    e._clear_pending()
     if due >= 0:
         e._avg_due[seat] = due
     assert e.modes == [nat.STRAT_F32, nat.STRAT_F32]

@@ -37,26 +37,15 @@ def _engine(spec, stack=STACK, **kw):
     return s
 
 
-def _pairing_engine(spec, immediate=False, **kw):
-    """test_gpu_board_avg_pairing._engine at the short stack: the immediate form writes each sweep's own averaging step"""
-    from pokerrl_b200 import _native as nat
-    from pokerrl_b200.board_engine import BoardCFRSolver, _stream
-
-    class Immediate(BoardCFRSolver):
-        def _sweep_begin(self, bufs, p, evaluate, src_own, src_opp):
-            nat.call("prl_board_sweep", C.byref(self.g), p, int(evaluate), src_own, src_opp, self._trunk_reach_row(bufs, 1 - p),
-                     self.iter_counter, self.delay, self.algo, 0.0, 0, _stream(self.device))
-
-    return (Immediate if immediate else BoardCFRSolver)(G, _args(STACK), spec, **kw)
-
-
 @pytest.fixture
 def at_stack(monkeypatch):
     """at_stack(s): the parity modules build their games at stack s"""
+    pairing_engine = pairing._engine
+
     def bind(stack=STACK):
         monkeypatch.setattr(eng, "_engine", functools.partial(_engine, stack=stack))
         monkeypatch.setattr(eng, "fhp_tree", functools.partial(fhp_tree, stack=stack))
-        monkeypatch.setattr(pairing, "_engine", _pairing_engine)
+        monkeypatch.setattr(pairing, "_engine", functools.partial(pairing_engine, args=_args(stack)))
         monkeypatch.setattr(brt, "STACK", [stack, stack])
     bind()
     return bind

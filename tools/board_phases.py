@@ -64,10 +64,8 @@ def main():
     torch.cuda.synchronize()
     t, stream = s.iter_counter, _stream(s.device)
     forms = {
-        "defer": lambda p: nat.call("prl_board_update_cfrp", C.byref(s.g), p, s._trunk_reach_row(s.bufs, 1 - p), t, s.delay, -1, 0,
-                                    stream),
-        "paired": lambda p: nat.call("prl_board_update_cfrp", C.byref(s.g), p, s._trunk_reach_row(s.bufs, 1 - p), t, s.delay, t - 1,
-                                     1, stream),
+        "defer": lambda p: s._board_update_cfrp(p, -1, 0),
+        "paired": lambda p: s._board_update_cfrp(p, t - 1, 1),
         "eval": lambda p: s._sweep_begin(s.bufs, p, True, 0, 0),
         "flush": lambda p: nat.call("prl_board_avg_flush", C.byref(s.g), p, t - 1, s.delay, stream),
     }

@@ -62,9 +62,8 @@ def per_launch_ms(launch, reps=10):
 # the forms of one seat's CFR+ update at iteration t (after this the solver's tables are no longer a CFR+ run)
 t, stream = s.iter_counter, _stream(s.device)
 forms = {
-    "defer": lambda p: nat.call("prl_board_update_cfrp", C.byref(s.g), p, s._trunk_reach_row(s.bufs, 1 - p), t, s.delay, -1, 0, stream),
-    "paired": lambda p: nat.call("prl_board_update_cfrp", C.byref(s.g), p, s._trunk_reach_row(s.bufs, 1 - p), t, s.delay, t - 1, 1,
-                                 stream),
+    "defer": lambda p: s._board_update_cfrp(p, -1, 0),
+    "paired": lambda p: s._board_update_cfrp(p, t - 1, 1),
     "flush": lambda p: nat.call("prl_board_avg_flush", C.byref(s.g), p, t - 1, s.delay, stream),
 }
 # a seat owns half of a board's rows: defer reads the opponent's and its own regrets and writes its own (3 halves), paired also
