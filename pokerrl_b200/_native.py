@@ -7,7 +7,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# PRL_LIB_PATH: another build of the same library (tools/build_variants.py writes kernel-variant builds for A/B timing)
+# PRL_LIB_PATH: another build of the same library (tools/build_variants.py stamps writes the phase-stamp build)
 LIB_PATH = os.environ.get("PRL_LIB_PATH") or os.path.join(_HERE, "lib", "libpokerrl_b200.so")
 
 # enums of include/pokerrl_b200.h

@@ -48,40 +48,16 @@ constexpr int kBlobA = kRecBytes + kShBytes;                // 10 880 B, needed 
 constexpr int kBlobBytes = kBlobA + kRowIdxBytes;           // 15 392 B
 static_assert(kBlobA % 16 == 0 && kRowIdxBytes % 16 == 0, "bulk copies move multiples of 16 bytes");
 
-// kernel variants (A/B switches, tools/build_variants.py; the defaults are the variants kept)
-#ifndef PRL_BV_RED
-#define PRL_BV_RED 1         // chance sums by 64-bit RED instead of load + add + store
-#endif
-#ifndef PRL_BV_P1PIPE
-#define PRL_BV_P1PIPE 1      // P1 rows: 1 = only the first position requested one unit ahead, the rest inside P1; 0 = all three
-#endif
-#ifndef PRL_BV_FOLDLIN
-#define PRL_BV_FOLDLIN 1     // update form: card-row sums of the fold vectors from the showdown vectors' row totals (linearity)
-#endif
-#ifndef PRL_BV_ERT
-#define PRL_BV_ERT 1         // card-row prefix arrays entry-major (Er[v][k][card]) instead of card-major: fewer store conflicts in P2a
-#endif
-#ifndef PRL_BV_ROWTOTF
-#define PRL_BV_ROWTOTF 1     // kLin: a lane's part of a card row's total summed in float (12 terms), only the quad reduction in double
-                             // (measured: +1 %, parity unchanged at <= 1.6e-7)
-#endif
-#ifndef PRL_BV_NEWTON
-#define PRL_BV_NEWTON 1      // regret matching: Newton step after MUFU.RCP (<= 1 ulp); 0 = the approximation as is (2^-23 relative)
-#endif
-#ifndef PRL_BV_PF
-#define PRL_BV_PF 1          // table rows into L2, update forms: 1 = each stream one phase ahead of its first use (own rows at B1
-                             // of their unit, the next unit's opponent rows at B2); 0 = all rows of the next board at the unit's top
-#endif
+// instrumentation switch, off in the library (tools/build_variants.py stamps builds it on)
 #ifndef PRL_BV_STAMPS
 #define PRL_BV_STAMPS 0      // 1 = phase stamps: clock64() at the unit start and B1-B5 of sampled units (tools/board_phases.py)
 #endif
-constexpr int kVP1Pipe = PRL_BV_P1PIPE;
-constexpr bool kVRed = PRL_BV_RED, kVFoldLin = PRL_BV_FOLDLIN, kVErT = PRL_BV_ERT;
-// tried and removed: five-warp / one-warp-per-vector scans, the single-warp stage spread
-// over nine warps, the third P3 pass spread over all warps, two positions requested a unit ahead
+// tried and removed: five-warp / one-warp-per-vector scans, the single-warp stage spread over nine warps, the third P3 pass
+// spread over all warps, two positions requested a unit ahead, all three positions requested a unit ahead, chance sums by
+// load + add + store, card-major card-row prefix arrays, row totals summed in double per element, the bare MUFU.RCP, fold
+// row sums gathered in the update forms, all rows of the next board prefetched at the top of an update unit (DESIGN §6.1)
 
 constexpr int kThreads = 384;  // 12 warps; 3 strength positions per thread (3 * 384 = 1152 >= 1081: 94 % of the lanes busy)
-constexpr int kPerThread = 3;
 constexpr int kWarps = kThreads / 32;
 
 // ---- compiled shapes of the post-deal subtree (breadth-first; Flop5Holdem with pot-size raises).  The host checks the game's
@@ -308,7 +284,7 @@ __device__ __forceinline__ void node_strategy(const float (&g)[A], int src, floa
     const float sm = fmaxf(sum, 1e-37f);
     float inv;
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv) : "f"(sm));
-    if (PRL_BV_NEWTON) inv = fmaf(inv, fmaf(-sm, inv, 1.0f), inv);
+    inv = fmaf(inv, fmaf(-sm, inv, 1.0f), inv);
     inv = pos ? inv : 0.0f;
     const float uni = pos ? 0.0f : 1.0f / (float)A;  // CFRPlus.py:53-58: uniform where no regret is positive
 #pragma unroll
@@ -354,7 +330,8 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + M::kBarOff);  // [0], [1]: blob A buffers; [2]: card rows
     const int16_t* rowidx = reinterpret_cast<const int16_t*>(smem + M::kRowIdxOff);
     double* rowtot = reinterpret_cast<double*>(smem + M::kRowTotOff);  // [NSD][48]
-    constexpr bool kLin = kVFoldLin && !EVAL;  // evaluation may read average-strategy rows, which sum to one only up to rounding
+    // kLin: card-row sums of the fold vectors from the showdown vectors' row totals (linearity), update forms only:
+    constexpr bool kLin = !EVAL;  // evaluation may read average-strategy rows, which sum to one only up to rounding
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const prl_board_game_t& G = a.g;
@@ -395,11 +372,11 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
         if (read_avg) bulk_prefetch_l2(G.avg + (size_t)jj * kBoardFloats + (size_t)OWN0 * kLdb, NOWN * kLdb * 4);
         if (defer_now) bulk_prefetch_l2(G.avg + (size_t)jj * kBoardFloats + (size_t)OPP0 * kLdb, NOPP * kLdb * 4);
     };
-    // Update forms (PRL_BV_PF): each stream one phase ahead of its first use, so that a CTA holds about one board's rows in L2,
-    // not two - two boards of the paired form (264 CTAs x (2 x 91 KB read + 61 KB stored)) overflow the 50 MB L2 of an H100,
-    // and rows evicted before their use are fetched twice.  The evaluation form stores nothing and fits two boards deep
-    // (31 MB): it keeps the whole-unit lead (measured: the phase schedule slowed it by 4 %).
-    constexpr bool kPfPhase = PRL_BV_PF && !EVAL;
+    // Update forms: each stream one phase ahead of its first use, so that a CTA holds about one board's rows in L2, not two -
+    // two boards of the paired form (264 CTAs x (2 x 91 KB read + 61 KB stored)) overflow the 50 MB L2 of an H100, and rows
+    // evicted before their use are fetched twice.  The evaluation form stores nothing and fits two boards deep (31 MB): it
+    // keeps the whole-unit lead (measured: the phase schedule slowed it by 4 %).
+    constexpr bool kPfPhase = !EVAL;
     // rows first read in P1: the next unit's opponent rows (DEFER: and the opponent's average rows), prefetched at B2 ...
     auto prefetch_opp = [&](int jj) {
         bulk_prefetch_l2(tab_opp + (size_t)jj * kBoardFloats + (size_t)OPP0 * kLdb, NOPP * kLdb * 4);
@@ -421,11 +398,10 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
         else prefetch_rows(j);
     }
 
-    // P1 inputs of the thread's three strength positions (opponent rows + trunk reach).  kVP1Pipe: only the first position
-    // is requested one unit ahead (8 registers live across the unit's last barrier - 24 spilled to local memory and made the
+    // P1 inputs of the thread's three strength positions (opponent rows + trunk reach).  Only the first position is
+    // requested one unit ahead (8 registers live across the unit's last barrier - 24 spilled to local memory and made the
     // warp wait for the loads there); the other two are requested inside P1, one position ahead of their use.
-    constexpr int kP1Ahead = kVP1Pipe ? kVP1Pipe : kPerThread;
-    float p1_g[kP1Ahead][NOPP], p1_x0[kP1Ahead];
+    float p1_g[NOPP], p1_x0;
     auto p1_load_k = [&](int jj, const int16_t* sh_jj, int k, float (&g)[NOPP], float& x0) {
         // lanes past the last hand read the last hand's values (never used): unconditional loads keep the arrays in registers
         const int i = min(tid + k * kThreads, kLive - 1);
@@ -434,10 +410,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
         for (int r = 0; r < NOPP; ++r) g[r] = ld_stream(rows + (size_t)r * kLdb);
         x0 = __ldg(a.trunk_reach_opp + sh_jj[i]);
     };
-    auto p1_load = [&](int jj, const int16_t* sh_jj) {
-#pragma unroll
-        for (int k = 0; k < kP1Ahead; ++k) p1_load_k(jj, sh_jj, k, p1_g[k], p1_x0[k]);
-    };
+    auto p1_load = [&](int jj, const int16_t* sh_jj) { p1_load_k(jj, sh_jj, 0, p1_g, p1_x0); };
 
     for (int it = 0; j < nb; j += gridDim.x, ++it) {
         const int buf = it & 1;
@@ -500,16 +473,13 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
                 });
             }
         };
-        if constexpr (kVP1Pipe == 1) {
+        {
             float gB[NOPP], gC[NOPP], xB = 0.0f, xC = 0.0f;
             p1_load_k(j, sh, 1, gB, xB);
-            p1_hand(0, p1_g[0], p1_x0[0]);
+            p1_hand(0, p1_g, p1_x0);
             p1_load_k(j, sh, 2, gC, xC);
             p1_hand(1, gB, xB);
             p1_hand(2, gC, xC);
-        } else {
-#pragma unroll
-            for (int k = 0; k < kPerThread; ++k) p1_hand(k, p1_g[k], p1_x0[k]);
         }
         __syncthreads();  // B1: S complete
         stamp(it, 1);
@@ -551,16 +521,15 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
                 const float* Sv = S + v * kLdb;
                 float inc[kRowSeg];
                 float run = 0.0f;
-                double drun = 0.0;  // kLin: the row's total in double (the fold vectors' row sums derive from these)
 #pragma unroll
                 for (int e = 0; e < kRowSeg; ++e) {
-                    const float xv = Sv[idx[e]];
                     inc[e] = run;
-                    run += xv;
-                    if constexpr (kLin && !PRL_BV_ROWTOTF) drun += (double)xv;
+                    run += Sv[idx[e]];
                 }
                 if constexpr (kLin) {
-                    if constexpr (PRL_BV_ROWTOTF) drun = (double)run;
+                    // the row's total in double (the fold vectors' row sums derive from these): a lane's 12 terms summed in
+                    // float, only the quad reduction in double (measured: +1 %, parity unchanged at <= 1.6e-7)
+                    double drun = (double)run;
                     drun += __shfl_xor_sync(qmask, drun, 1, 4);
                     drun += __shfl_xor_sync(qmask, drun, 2, 4);
                     if (row_live && q == 0) rowtot[v * kRowPad + lc] = drun;
@@ -572,10 +541,10 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
                 if (q >= 2) sc += tt;
                 const float half = 0.5f * __shfl_sync(qmask, sc, 3, 4);
                 const float off = (sc - run) - half;
-                float* row = Er + v * kErVec + (kVErT ? q * kRowSeg * kErStride + lc : lc * kErStride + q * kRowSeg);
+                float* row = Er + v * kErVec + q * kRowSeg * kErStride + lc;  // entry-major: Er[v][k][card]
 #pragma unroll
                 for (int e = 0; e < kRowSeg; ++e)
-                    if (row_live && q * kRowSeg + e < kErStride) row[kVErT ? e * kErStride : e] = off + inc[e];
+                    if (row_live && q * kRowSeg + e < kErStride) row[e * kErStride] = off + inc[e];
             }
 #pragma unroll 1
             for (int f = kFoldSplit * grp; f < (kLin ? 0 : kFoldSplit * grp + kFoldSplit); ++f) {  // kLin: nothing to gather for the fold vectors
@@ -707,16 +676,11 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
             const uint64_t w = rec[i];
             const int hand = sh[i];
             long long* wacc = wp + hand;
-            long long w_ev = 0, w_br = 0;
-            if constexpr (!kVRed) {
-                w_ev = *wacc;
-                if constexpr (EVAL) w_br = wacc[kRange];
-            }
             const int gs = (int)(w & 0x7ffu), ge = (int)((w >> 11) & 0x7ffu);
             const int lc1 = (int)((w >> 22) & 0x3fu), lc2 = (int)((w >> 28) & 0x3fu);
             const int k1 = (int)((w >> 34) & 0x3fu), t1 = (int)((w >> 40) & 0x3fu), k2 = (int)((w >> 46) & 0x3fu), t2 = (int)((w >> 52) & 0x3fu);
-            const int o1 = kVErT ? k1 * kErStride + lc1 : lc1 * kErStride + k1, o1e = o1 + (kVErT ? t1 * kErStride : t1);
-            const int o2 = kVErT ? k2 * kErStride + lc2 : lc2 * kErStride + k2, o2e = o2 + (kVErT ? t2 * kErStride : t2);
+            const int o1 = k1 * kErStride + lc1, o1e = o1 + t1 * kErStride;
+            const int o2 = k2 * kErStride + lc2, o2e = o2 + t2 * kErStride;
             float e[SH::N], br[EVAL ? SH::N : 1];
             // terminal rows (ValueFiller.py:103-158): ev = equity * K * pot / 2, the folder loses
             static_for<0, SH::N>([&](auto I) {
@@ -790,15 +754,11 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
                     }
                 }
             });
-            // the board's contribution to its parent's sum (ValueFiller.py:76-78), 64-bit fixed point
-            if constexpr (kVRed) {  // fire-and-forget 64-bit RED into the CTA's private vector: nothing to wait for
-                atomicAdd(reinterpret_cast<unsigned long long*>(wacc), (unsigned long long)__double2ll_rn((double)e[0] * fx));
-                if constexpr (EVAL)
-                    atomicAdd(reinterpret_cast<unsigned long long*>(wacc + kRange), (unsigned long long)__double2ll_rn((double)br[0] * fx));
-            } else {
-                *wacc = w_ev + __double2ll_rn((double)e[0] * fx);
-                if constexpr (EVAL) wacc[kRange] = w_br + __double2ll_rn((double)br[0] * fx);
-            }
+            // the board's contribution to its parent's sum (ValueFiller.py:76-78), 64-bit fixed point: fire-and-forget 64-bit RED
+            // into the CTA's private vector, nothing to wait for
+            atomicAdd(reinterpret_cast<unsigned long long*>(wacc), (unsigned long long)__double2ll_rn((double)e[0] * fx));
+            if constexpr (EVAL)
+                atomicAdd(reinterpret_cast<unsigned long long*>(wacc + kRange), (unsigned long long)__double2ll_rn((double)br[0] * fx));
         };
         // software pipeline over the thread's three strength positions: the next position's rows are in flight while the
         // current one is evaluated (position 0 was requested before the prefix sums were written back)

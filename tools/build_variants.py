@@ -1,6 +1,6 @@
-"""A/B builds of the board sweep kernel: python tools/build_variants.py
-Compiles csrc/cfr_board.cu with different PRL_BV_* switches into pokerrl_b200/lib/variants/lib_<name>.so (the other
-translation units are taken from the regular build); run one with PRL_LIB_PATH=<that file> python tools/board_probe.py."""
+"""Phase-stamp build of the board sweep kernel: python tools/build_variants.py stamps
+Compiles csrc/cfr_board.cu with PRL_BV_STAMPS=1 into pokerrl_b200/lib/variants/lib_stamps.so (the other translation units
+are taken from the regular build); run it with PRL_LIB_PATH=<that file> python tools/board_phases.py."""
 import os
 import subprocess
 import sys
@@ -9,22 +9,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from pokerrl_b200.csrc import build as B  # noqa: E402
 
-# switches left in csrc/cfr_board.cu: each accepted change against its predecessor (the rejected ones were removed from the
-# source)
-_ON = dict(RED=1, P1PIPE=1, FOLDLIN=1, ERT=1, ROWTOTF=1, NEWTON=1, PF=1, STAMPS=0)
 VARIANTS = {
-    "final": dict(_ON),
-    "base": dict(RED=0, P1PIPE=0, FOLDLIN=0, ERT=0, ROWTOTF=0, NEWTON=1, PF=0, STAMPS=0),
-    "no_red": dict(_ON, RED=0),
-    "no_p1pipe": dict(_ON, P1PIPE=0),
-    "no_foldlin": dict(_ON, FOLDLIN=0),
-    "no_ert": dict(_ON, ERT=0),
-    "no_rowtotf": dict(_ON, ROWTOTF=0),
-    "no_newton": dict(_ON, NEWTON=0),
-    "pf0": dict(_ON, PF=0),
-    # phase stamps (tools/board_phases.py) of the kept schedule and of the previous one
-    "stamps": dict(_ON, STAMPS=1),
-    "stamps_pf0": dict(_ON, PF=0, STAMPS=1),
+    "stamps": dict(STAMPS=1),  # phase stamps (tools/board_phases.py)
 }
 
 
