@@ -29,8 +29,9 @@ typedef void* prl_stream_t; /* cudaStream_t */
    (2: prl_tree_t gained board_hand_rec / node_rec2 / work_rec2 / level_nfold; 3: board engine, legacy LUT natives;
     4: prl_board_sweep / prl_board_trunk take the algorithm; prl_tree_t gained the all-in terminals of two-card games: level_nallin / allin_nodes / allin_pot / allin_tiles /
     allin_partial; 5: prl_board_update_cfrp / prl_board_avg_flush; 6: prl_board_policy_query; 7: second board-engine shape,
-    prl_board_layout / prl_board_rows / prl_board_policy_query take the shape) */
-#define PRL_ABI_VERSION 7
+    prl_board_layout / prl_board_rows / prl_board_policy_query take the shape; 8: PRL_ALGO_DCFR, prl_buffers_t / prl_board_game_t
+    gained the DCFR factor table `dcfr`) */
+#define PRL_ABI_VERSION 8
 
 /* node kinds (game/_/tree/_/nodes.py:8-62 + ValueFiller.py:34-62) */
 enum {
@@ -42,8 +43,11 @@ enum {
     PRL_KIND_SHOWDOWN_ALLIN = 5  /* terminal: all-in showdown before the board is complete */
 };
 
-/* algorithms (cfr/VanillaCFR.py, cfr/CFRPlus.py, cfr/LinearCFR.py) */
-enum { PRL_ALGO_VANILLA = 0, PRL_ALGO_CFR_PLUS = 1, PRL_ALGO_LINEAR = 2 };
+/* algorithms (cfr/VanillaCFR.py, cfr/CFRPlus.py, cfr/LinearCFR.py; Discounted CFR, Brown & Sandholm, AAAI 2019).
+ * DCFR, iteration counter i, t = i + 1, factors {a_t, b_t, w_t} = row i of the caller's table `dcfr`: seat p's regret
+ * update is x = d + R_old, R_new = x * (x > 0 ? a_t : b_t), the strategy is regret matching of R_new and the average is the
+ * reach-weighted sum of strategies with weight w_t (as Linear CFR's with weight t). */
+enum { PRL_ALGO_VANILLA = 0, PRL_ALGO_CFR_PLUS = 1, PRL_ALGO_LINEAR = 2, PRL_ALGO_DCFR = 3 };
 
 /* where a player's strategy comes from in a reach / value pass, and in which precision the reference computes
  * with it (SURVEY.md appendix C) */
@@ -137,6 +141,8 @@ typedef struct {
     void* avg;     /* DEVICE float|double[n_slots][ld]  node.data["avg_strat"] (CFR+) / ["avg_strat_sum"] */
     void* workspace;          /* DEVICE scratch for the chance-node reductions of two-card games (else NULL) */
     uint64_t workspace_bytes; /* >= 4 * n_chance_per_level * (ceil(max_chance_children / 128) + 1) * ld * 4 bytes */
+    const float* dcfr;        /* DEVICE float[n][3] {a_t, b_t, w_t}, row = iteration counter (n > every counter a call
+                                 updates with); read by PRL_ALGO_DCFR only, which fails without it (NULL otherwise) */
 } prl_buffers_t;
 
 /* library info */
@@ -259,6 +265,7 @@ typedef struct {
     int64_t* w_total;        /* DEVICE int64[4][n_range]: fixed-point sums over this device's boards of board_mult * root value,
                                 natural hand order.  Update sweep: array 0 = ev of the seat; evaluation sweep of seat p:
                                 arrays 2p = ev, 2p + 1 = ev_br */
+    const float* dcfr;       /* DEVICE float[n][3] {a_t, b_t, w_t} of PRL_ALGO_DCFR as in prl_buffers_t (NULL otherwise) */
 } prl_board_game_t;
 
 /* out[8] = {n_live, ldb, blob bytes per board, byte offset of the int16 hand ids, byte offset of the card rows,
@@ -284,7 +291,8 @@ int prl_board_build_tables(const int32_t* ranks, const uint64_t* board_mask, con
  * Vanilla / Linear CFR (VanillaCFR.py:54-60, LinearCFR.py:53-59): the average is the sum of strategy x own reach x weight with
  * the reach under the NEW strategy, trunk included - known only after the seat's trunk update.  The contribution of the
  * OPPONENT's last update is therefore added by this sweep (defer_w = its weight, 0 = none pending), which walks those rows
- * anyway; p1_only != 0 does nothing else (flush before the average strategy is evaluated or exported). */
+ * anyway; p1_only != 0 does nothing else (flush before the average strategy is evaluated or exported).  DCFR takes the same
+ * deferred path, with defer_w = the w_t of the iteration of the opponent's update. */
 int prl_board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, int src_opp, const float* trunk_reach_opp,
                     int iter, int delay, int algo, float defer_w, int p1_only, prl_stream_t stream);
 

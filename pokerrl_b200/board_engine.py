@@ -17,12 +17,13 @@ import numpy as np
 import torch
 
 from pokerrl_b200 import _native as nat
+from pokerrl_b200 import dcfr as _dcfr
 from pokerrl_b200.game.flat_tree import FlatTree
 from pokerrl_b200.game.holdem_boards import BoardSpec
 from pokerrl_b200.solver import DeviceTree, TreeBuffers, TreeOps, _require_cuda
 
 SRC_REGRET, SRC_AVG, SRC_AVG_SUM = 0, 1, 2
-ALGOS = {"VanillaCFR": nat.ALGO_VANILLA, "CFRPlus": nat.ALGO_CFR_PLUS, "LinearCFR": nat.ALGO_LINEAR}
+ALGOS = {"VanillaCFR": nat.ALGO_VANILLA, "CFRPlus": nat.ALGO_CFR_PLUS, "LinearCFR": nat.ALGO_LINEAR, "DCFR": nat.ALGO_DCFR}
 
 
 def board_layout(g=None):
@@ -270,10 +271,12 @@ class _BoardEngine:
 
 class BoardCFRSolver(_BoardEngine):
     def __init__(self, game_cls, env_args, board_spec=None, algo="CFRPlus", delay=0, device=None, rank=0, world=1,
-                 group=None, grid=0, reduce_fn=None):
+                 group=None, grid=0, reduce_fn=None, dcfr=_dcfr.DEFAULT):
         if algo not in ALGOS:
             raise ValueError("unknown algorithm %r" % (algo,))
+        self.dcfr = _dcfr.check_params(*dcfr) if algo == "DCFR" else None
         self.device = _require_cuda(device)
+        self._factors = _dcfr.FactorTable(self.dcfr, self.device) if self.dcfr else None
         self.rank, self.world, self.group = int(rank), int(world), group
         # cross-rank sum of the fixed-point chance sums, in place; default: torch.distributed all-reduce when world > 1
         self._reduce_fn = reduce_fn
@@ -336,7 +339,7 @@ class BoardCFRSolver(_BoardEngine):
     # ------------------------------------------------------------------------------------------------ helpers
     def _clear_pending(self):
         """no average-strategy update pending on either seat.
-        _pending (Vanilla / Linear CFR): weight of the average-strategy contribution of each seat's last update that the
+        _pending (Vanilla / Linear CFR, DCFR): weight of the average-strategy contribution of each seat's last update that the
         post-deal rows have not received yet (it is added by the next sweep that walks those rows: csrc/cfr_board.cu, DEFER).
         _avg_due (CFR+): iteration of each seat's averaging step that is still pending (-1: none).  An update sweep with
         nothing pending leaves its step pending; the seat's next update sweep applies it together with its own
@@ -434,8 +437,11 @@ class BoardCFRSolver(_BoardEngine):
         cl = self.chance_level
         if self.algo != nat.ALGO_CFR_PLUS:  # VanillaCFR.py:56-59 / LinearCFR.py:55-58: weight of this update's strategy in the sums
             if not self.fused_trunk:
-                raise RuntimeError("Vanilla / Linear CFR on the board engine need the fused trunk (unset PRL_TRUNK=levels)")
-            self._pending[p] = float(self.iter_counter + 1) if self.algo == nat.ALGO_LINEAR else 1.0
+                raise RuntimeError("Vanilla / Linear CFR and DCFR on the board engine need the fused trunk (unset PRL_TRUNK=levels)")
+            if self.algo == nat.ALGO_DCFR:  # w_t of THIS iteration, whichever later sweep adds the contribution
+                self._pending[p] = self._factors.w(self.iter_counter)
+            else:
+                self._pending[p] = float(self.iter_counter + 1) if self.algo == nat.ALGO_LINEAR else 1.0
         if self.fused_trunk:
             self._reduce(self.w_total[:1])
             self._trunk(self.bufs, self.modes, False, p)
@@ -461,6 +467,8 @@ class BoardCFRSolver(_BoardEngine):
 
     def iteration(self, n=1):
         with torch.cuda.device(self.device):
+            if self._factors is not None:  # DCFR: the factor table covers the next n iterations
+                self.g.dcfr = self._factors.ensure(self.iter_counter + n)
             for _ in range(n):
                 for p in (0, 1):  # _CFRBase.py:122-128
                     self._update_begin(p)
@@ -547,14 +555,16 @@ class BoardCFRSolver(_BoardEngine):
 
     def state_dict(self):
         self.flush_average()
-        return {"engine": "board", "algo": self.algo_name, "delay": self.delay, "iter_counter": self.iter_counter,
+        return {"engine": "board", "algo": self.algo_name, "delay": self.delay, "dcfr": list(self.dcfr) if self.dcfr else None,
+                "iter_counter": self.iter_counter,
                 "modes": list(self.modes), "rank": self.rank, "world": self.world, "n_boards": self.n_boards,
                 "n_boards_total": self.n_boards_total, "regret": self.regret.cpu(), "avg": self.avg.cpu(),
                 "trunk_regret": self.bufs.regret.cpu(), "trunk_strat": self.bufs.strat.cpu(), "trunk_avg": self.bufs.avg.cpu()}
 
     def load_state_dict(self, state):
-        for k in ("engine", "algo", "delay", "rank", "world", "n_boards", "n_boards_total"):
-            mine = {"engine": "board", "algo": self.algo_name}.get(k, getattr(self, k, None))
+        for k in ("engine", "algo", "delay", "dcfr", "rank", "world", "n_boards", "n_boards_total"):
+            mine = {"engine": "board", "algo": self.algo_name, "dcfr": list(self.dcfr) if self.dcfr else None}.get(
+                k, getattr(self, k, None))
             if state.get(k) != mine:
                 raise ValueError("checkpoint mismatch on %r: file has %r, this solver %r" % (k, state.get(k), mine))
         if tuple(state["regret"].shape) != tuple(self.regret.shape):

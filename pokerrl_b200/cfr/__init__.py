@@ -1,0 +1,3 @@
+from pokerrl_b200.cfr.DiscountedCFR import DiscountedCFR
+
+__all__ = ["DiscountedCFR"]

@@ -191,7 +191,7 @@ struct SweepSmem {
     static constexpr int kRowTotOff = kMiscOff + kMiscBytes;                // double rowtot[n_sd][48]: card-row totals of the showdown vectors
     static constexpr int kRowTotBytes = SH::n_sd * kRowPad * 8;
     static constexpr int kBarOff = kRowTotOff + kRowTotBytes;               // 3 mbarriers
-    static constexpr int kSmemBytes = kBarOff + 32;
+    static constexpr int kSmemBytes = kBarOff + 32;                         // 3 mbarriers, then DCFR's {a_t, b_t}
     static_assert(kBlobOff % 16 == 0 && kRowIdxOff % 16 == 0 && kCsdOff % 8 == 0 && kMiscOff % 8 == 0 && kRowTotOff % 8 == 0 &&
                       kBarOff % 8 == 0, "alignment");
     static_assert(2 * (kSmemBytes + 1024) <= 233472, "two CTAs per SM (228 KB of shared memory per H100 SM)");
@@ -208,6 +208,7 @@ struct SweepArgs {
     int src_own, src_opp;          // evaluation: 0 = regret matching of `regret`, 1 = `avg` rows as they are (CFR+ average),
                                    // 2 = `avg` rows normalised (reach-weighted sums of Vanilla / Linear CFR, LinearCFR.py:64-71)
     float rw;                      // weight of the instantaneous regret: 1, Linear CFR iter + 1 (LinearCFR.py:27-28)
+    const float* disc;             // DEFER: DCFR's {a_t, b_t} of this iteration (device), nullptr: no discount
     float defer_w;                 // DEFER: weight of the opponent's pending average-strategy contribution (0: none)
     double fx_scale;               // 2^frac_bits
     float sc[16];                  // terminal n: K * pot / 2, negated where the seat of this sweep is the folder
@@ -350,6 +351,9 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
     const bool do_avg = !EVAL && !DEFER && AVG && a.iter >= a.delay;
     const bool pair = do_avg && a.pair;
     const bool defer_now = DEFER && a.defer_w != 0.0f;
+    // DCFR's {a_t, b_t} (DEFER with a.disc only) in the 8 spare bytes after the three mbarriers: read from shared memory where
+    // they are used, so that they occupy no register across the board loop (the DEFER form is at the register cap)
+    float* disc = reinterpret_cast<float*>(smem + M::kBarOff + 3 * sizeof(uint64_t));
     const bool read_avg = do_avg && (pair ? a.m_old_due : a.m_old) != 0.0f;  // the first step applied reads the stored average
 
     // private chance-sum accumulators of this CTA (global, L2-resident): [2][kRange] int64
@@ -362,6 +366,10 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
         mbar_init(&bars[1], 1);
         mbar_init(&bars[2], 1);
         fence_async_shared();
+        if (DEFER && a.disc) {
+            disc[0] = a.disc[0];
+            disc[1] = a.disc[1];
+        }
     }
     __syncthreads();
     int j = blockIdx.x;
@@ -739,8 +747,11 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
                         } else {
 #pragma unroll
                             for (int c = 0; c < A; ++c) {
-                                if constexpr (DEFER) g[c] = __fadd_rn(__fmul_rn(a.rw, e[fc + c] - v), g[c]);  // VanillaCFR.py:26-27, LinearCFR.py:27-28
-                                else g[c] = fmaxf((e[fc + c] - v) + g[c], 0.0f);                          // CFRPlus.py:37-41
+                                if constexpr (DEFER) {  // VanillaCFR.py:26-27, LinearCFR.py:27-28
+                                    g[c] = __fadd_rn(__fmul_rn(a.rw, e[fc + c] - v), g[c]);
+                                    // DCFR: the new sum times a_t where it is positive, else b_t
+                                    if (a.disc) g[c] = __fmul_rn(g[c], (g[c] > 0.0f) ? disc[0] : disc[1]);
+                                } else g[c] = fmaxf((e[fc + c] - v) + g[c], 0.0f);                          // CFRPlus.py:37-41
                             }
                             if constexpr (!DEFER) node_strategy<A>(g, 0, s);
 #pragma unroll
@@ -1055,7 +1066,7 @@ __global__ void __launch_bounds__(kTrunkThreads) trunk_kernel(const prl_trunk_t 
                                                               long long peer_offset, long long* __restrict__ w_scratch,
                                                               const int16_t* __restrict__ sym_perm, int n_sym, double inv_scale,
                                                               int p_upd, int iter, int delay, float m_old, float m_new, int algo,
-                                                              float rw, float* out_expl) {
+                                                              float rw, const float* __restrict__ disc, float* out_expl) {
     __shared__ float ro[kRange + 2];
     __shared__ float cs[64];
     __shared__ float red[32];
@@ -1149,7 +1160,8 @@ __global__ void __launch_bounds__(kTrunkThreads) trunk_kernel(const prl_trunk_t 
                         for (int c = 0; c < A; ++c) {
                             float* rg = t.regret + (size_t)(fs + c) * ld + h;
                             const float d = ev_p[(size_t)(fc + c) * ld + h] - v;
-                            const float r = (algo == PRL_ALGO_CFR_PLUS) ? fmaxf(d + *rg, 0.0f) : __fadd_rn(__fmul_rn(rw, d), *rg);
+                            float r = (algo == PRL_ALGO_CFR_PLUS) ? fmaxf(d + *rg, 0.0f) : __fadd_rn(__fmul_rn(rw, d), *rg);
+                            if (disc) r = __fmul_rn(r, (r > 0.0f) ? disc[0] : disc[1]);  // DCFR: a_t / b_t
                             *rg = r;
                             ssum += fmaxf(r, 0.0f);
                         }
@@ -1181,7 +1193,8 @@ __global__ void __launch_bounds__(kTrunkThreads) trunk_kernel(const prl_trunk_t 
                     if (k == p) {
                         s = t.strat[(size_t)(fs + c) * ld + h];
                         float* a = t.avg + (size_t)(fs + c) * ld + h;
-                        if (algo != PRL_ALGO_CFR_PLUS) *a = __fadd_rn(*a, __fmul_rn(__fmul_rn(s, r), rw));  // VanillaCFR.py:56-59, LinearCFR.py:55-58
+                        if (algo != PRL_ALGO_CFR_PLUS)  // VanillaCFR.py:56-59, LinearCFR.py:55-58; DCFR: weight w_t
+                            *a = __fadd_rn(*a, __fmul_rn(__fmul_rn(s, r), disc ? disc[2] : rw));
                         else if (iter >= delay) *a = m_old * (*a) + m_new * s;
                     }
                     rp[(size_t)(fc + c) * ld + h] = s * r;
@@ -1312,7 +1325,9 @@ extern "C" int prl_board_build_tables(const int32_t* ranks, const uint64_t* boar
 // written, 0: it is left pending.  Today's form (-1, 1), deferred (-1, 0), paired (due, 1).
 static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, int src_opp, const float* trunk_reach_opp, int iter,
                        int delay, int algo, float defer_w, int p1_only, int due, int now, prl_stream_t stream) {
-    if (algo != PRL_ALGO_CFR_PLUS && algo != PRL_ALGO_VANILLA && algo != PRL_ALGO_LINEAR) return prl::fail("prl_board_sweep: bad algo");
+    if (algo < PRL_ALGO_VANILLA || algo > PRL_ALGO_DCFR) return prl::fail("prl_board_sweep: bad algo");
+    if (algo == PRL_ALGO_DCFR && !eval && !p1_only && !g->dcfr)
+        return prl::fail("prl_board_sweep: DCFR needs the factor table g->dcfr");
     const bool defer = !eval && algo != PRL_ALGO_CFR_PLUS;
     if (p1_only && !defer) return prl::fail("prl_board_sweep: p1_only is the average flush of Vanilla / Linear CFR");
     const int layout_ok = with_shape(g, [&](auto sh) { return layout_matches<decltype(sh)>(g) ? 1 : 0; });
@@ -1339,6 +1354,7 @@ static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, 
     a.src_own = src_own;
     a.src_opp = src_opp;
     a.rw = (algo == PRL_ALGO_LINEAR) ? (float)(iter + 1) : 1.0f;
+    a.disc = (algo == PRL_ALGO_DCFR && !eval && !p1_only) ? g->dcfr + 3 * (size_t)iter : nullptr;
     a.defer_w = defer ? defer_w : 0.0f;
     a.fx_scale = (double)(1ull << g->frac_bits);
     for (int n = 0; n < 16; ++n) {
@@ -1459,8 +1475,10 @@ extern "C" int prl_board_policy_query(const prl_board_game_t* shape, const float
 extern "C" int prl_board_trunk(const prl_board_game_t* g, const prl_trunk_t* t, int eval, int p, int n_sym, const int16_t* sym_perm,
                                int iter, int delay, float* out_expl, const int64_t* const* peers, int n_peers,
                                int64_t peer_offset, int64_t* w_scratch, int algo, prl_stream_t stream) {
-    if (algo != PRL_ALGO_CFR_PLUS && algo != PRL_ALGO_VANILLA && algo != PRL_ALGO_LINEAR) return prl::fail("prl_board_trunk: bad algo");
+    if (algo < PRL_ALGO_VANILLA || algo > PRL_ALGO_DCFR) return prl::fail("prl_board_trunk: bad algo");
+    if (algo == PRL_ALGO_DCFR && !eval && (!g || !g->dcfr)) return prl::fail("prl_board_trunk: DCFR needs the factor table g->dcfr");
     const float rw = (algo == PRL_ALGO_LINEAR) ? (float)(iter + 1) : 1.0f;
+    const float* disc = (algo == PRL_ALGO_DCFR && !eval) ? g->dcfr + 3 * (size_t)iter : nullptr;
     if (!g || !t || t->n_nodes < 1 || t->n_nodes > 8) return prl::fail("prl_board_trunk: 1..8 trunk nodes");
     if (with_shape(g, [](auto) { return 0; }) == kNoShape) return prl::fail("prl_board_trunk: the post-deal subtree has no compiled shape");
     if (t->n_range != kRange || g->n_deck != kDeck) return prl::fail("prl_board_trunk: 52-card deck / 1326 hands only");
@@ -1477,10 +1495,10 @@ extern "C" int prl_board_trunk(const prl_board_game_t* g, const prl_trunk_t* t, 
     long long* ws = reinterpret_cast<long long*>(w_scratch);
     if (eval)
         trunk_kernel<true><<<1, kTrunkThreads, 0, (cudaStream_t)stream>>>(*t, w, pp, n_peers, (long long)peer_offset, ws, sym_perm, n_sym,
-                                                                       inv_scale, -1, iter, delay, m_old, m_new, algo, rw, out_expl);
+                                                                       inv_scale, -1, iter, delay, m_old, m_new, algo, rw, disc, out_expl);
     else
         trunk_kernel<false><<<1, kTrunkThreads, 0, (cudaStream_t)stream>>>(*t, w, pp, n_peers, (long long)peer_offset, ws, sym_perm, n_sym,
-                                                                        inv_scale, p, iter, delay, m_old, m_new, algo, rw, out_expl);
+                                                                        inv_scale, p, iter, delay, m_old, m_new, algo, rw, disc, out_expl);
     prl::count_launch();
     return prl::check(cudaGetLastError(), "prl_board_trunk");
 }

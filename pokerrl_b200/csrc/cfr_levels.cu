@@ -210,7 +210,7 @@ __device__ __forceinline__ void reach_group(const Ctx& c, const int lo, const in
                 const bool avg_f64 = upd && c.algo == PRL_ALGO_CFR_PLUS && c.avg_f64 && c.iter >= c.delay;
                 float* avf = (float*)c.B.avg + (size_t)fs * ld + h;
                 double* avd = (double*)c.B.avg + (size_t)fs * ld + h;
-                const float w = (float)(c.iter + 1);
+                const float w = (upd && c.algo == PRL_ALGO_DCFR) ? c.B.dcfr[3 * (size_t)c.iter + 2] : (float)(c.iter + 1);
                 for (int k0 = 0; k0 < A; k0 += kChunk) {  // loads of a chunk first, then the stores
                     float s[kChunk], av[kChunk];
                     double ad[kChunk];
@@ -232,7 +232,7 @@ __device__ __forceinline__ void reach_group(const Ctx& c, const int lo, const in
                             } else if (avg_f32) {
                                 float a;
                                 if (c.algo == PRL_ALGO_CFR_PLUS) a = (float)m_old * av[j] + (float)m_new * s[j];
-                                else if (c.algo == PRL_ALGO_LINEAR) a = av[j] + x * w;  // LinearCFR.py:56-61
+                                else if (c.algo == PRL_ALGO_LINEAR || c.algo == PRL_ALGO_DCFR) a = av[j] + x * w;  // LinearCFR.py:56-61
                                 else a = av[j] + x;                                      // VanillaCFR.py:57-62
                                 avf[(size_t)(k0 + j) * ld] = a;
                             }
@@ -310,9 +310,26 @@ __device__ __forceinline__ float fold_children(const float* __restrict__ col, in
     return v;
 }
 
-__device__ __forceinline__ float regret_step(int algo, float d, float old, float w) {
+// weights of the regret update of iteration c.iter: Linear CFR's iter + 1, DCFR's discounts of positive / negative sums
+struct RegretW {
+    float w, a, b;
+};
+__device__ __forceinline__ RegretW regret_w(const Ctx& c) {
+    RegretW r{(float)(c.iter + 1), 1.0f, 1.0f};
+    if (c.algo == PRL_ALGO_DCFR) {
+        r.a = c.B.dcfr[3 * (size_t)c.iter];
+        r.b = c.B.dcfr[3 * (size_t)c.iter + 1];
+    }
+    return r;
+}
+
+__device__ __forceinline__ float regret_step(int algo, float d, float old, const RegretW& w) {
     if (algo == PRL_ALGO_CFR_PLUS) return fmaxf(d + old, 0.0f);  // CFRPlus.py:37-41
-    if (algo == PRL_ALGO_LINEAR) return w * d + old;             // LinearCFR.py:27-31
+    if (algo == PRL_ALGO_LINEAR) return w.w * d + old;           // LinearCFR.py:27-31
+    if (algo == PRL_ALGO_DCFR) {                                 // discounted after this iteration's regret is added
+        const float x = d + old;
+        return x * ((x > 0.0f) ? w.a : w.b);
+    }
     return d + old;                                              // VanillaCFR.py:26-30
 }
 
@@ -344,7 +361,7 @@ __device__ __forceinline__ float update_own(const Ctx& c, int md, const float* _
         for (int k = 1; k < A; ++k) acc = acc + strat_f64(c, md, fs, k, A, h) * (double)e[k];
         v = (float)acc;
     }
-    const float w = (float)(c.iter + 1);
+    const RegretW w = regret_w(c);
     float ssum = 0.0f;
 #pragma unroll
     for (int k = 0; k < A; ++k) {
@@ -437,7 +454,7 @@ __device__ __forceinline__ void value_group(const Ctx& c, const int lo, const in
                 if (upd) {  // wide node: stream (regrets are recomputed in the second loop instead of re-read)
                     float* rcol = c.B.regret + (size_t)fs * ld + h;
                     float* scol = c.B.strat + (size_t)fs * ld + h;
-                    const float w = (float)(c.iter + 1);
+                    const RegretW w = regret_w(c);
                     float ssum = 0.0f;
                     for (int k = 0; k < A; ++k) {
                         const float rp = fmaxf(regret_step(c.algo, ecol[(size_t)k * ld] - v, rcol[(size_t)k * ld], w), 0.0f);
@@ -672,7 +689,8 @@ extern "C" int prl_cfr_sweep(const prl_tree_t* tree, const prl_buffers_t* buf, i
         return prl2::cfr_sweep(tree, buf, algo, p, iter, delay, strat_mode, which, (cudaStream_t)stream);
     }
     if (int e = check_tree(tree)) return e;
-    if (p < 0 || p > 1 || algo < 0 || algo > 2) return prl::fail("prl_cfr_sweep: bad p / algo");
+    if (p < 0 || p > 1 || algo < 0 || algo > 3) return prl::fail("prl_cfr_sweep: bad p / algo");
+    if (algo == PRL_ALGO_DCFR && !buf->dcfr) return prl::fail("prl_cfr_sweep: DCFR needs the factor table buf->dcfr");
     if (algo != PRL_ALGO_CFR_PLUS && avg_f64) return prl::fail("avg_f64 only applies to CFR+");
     Ctx c{*tree, *buf, 0, 0, 1 << p, {strat_mode[0], strat_mode[1]}, algo, p, iter, delay, avg_f64};
     if (which & 1) value_sweep(c, false, true, (cudaStream_t)stream);
@@ -750,7 +768,8 @@ extern "C" int prl_cfr_iterations(const prl_tree_t* tree, const prl_buffers_t* b
         return 0;
     }
     if (int e = check_tree(tree)) return e;
-    if (algo < 0 || algo > 2 || n_iters < 0) return prl::fail("prl_cfr_iterations: bad algo / n_iters");
+    if (algo < 0 || algo > 3 || n_iters < 0) return prl::fail("prl_cfr_iterations: bad algo / n_iters");
+    if (algo == PRL_ALGO_DCFR && !buf->dcfr) return prl::fail("prl_cfr_iterations: DCFR needs the factor table buf->dcfr");
     if (algo != PRL_ALGO_CFR_PLUS && avg_f64) return prl::fail("avg_f64 only applies to CFR+");
     if (n_iters == 0) return 0;
     Ctx c{*tree, *buf, 0, 0, 0, {strat_mode[0], strat_mode[1]}, algo, 0, iter0, delay, avg_f64};

@@ -88,10 +88,27 @@ __device__ __forceinline__ bool hand_blocked(const prl_tree_t& T, int h, unsigne
 }
 
 // ------------------------------------------------------------------------------------------------ CFR rules
-// new regret of one (row, hand) from the instantaneous regret d = v(child) - v(node) and the stored regret; w = iter + 1
-__device__ __forceinline__ float regret_step(int algo, float d, float old, float w) {
+// weights of the regret update of iteration c.iter: Linear CFR's iter + 1, DCFR's discounts of positive / negative sums
+struct RegretW {
+    float w, a, b;
+};
+__device__ __forceinline__ RegretW regret_w(const Ctx2& c) {
+    RegretW r{(float)(c.iter + 1), 1.0f, 1.0f};
+    if (c.algo == PRL_ALGO_DCFR) {
+        r.a = c.B.dcfr[3 * (size_t)c.iter];
+        r.b = c.B.dcfr[3 * (size_t)c.iter + 1];
+    }
+    return r;
+}
+
+// new regret of one (row, hand) from the instantaneous regret d = v(child) - v(node) and the stored regret
+__device__ __forceinline__ float regret_step(int algo, float d, float old, const RegretW& w) {
     if (algo == PRL_ALGO_CFR_PLUS) return fmaxf(d + old, 0.0f);
-    if (algo == PRL_ALGO_LINEAR) return w * d + old;
+    if (algo == PRL_ALGO_LINEAR) return w.w * d + old;
+    if (algo == PRL_ALGO_DCFR) {  // discounted after this iteration's regret is added
+        const float x = d + old;
+        return x * ((x > 0.0f) ? w.a : w.b);
+    }
     return d + old;
 }
 
@@ -123,7 +140,8 @@ __device__ __forceinline__ void avg_update(const Ctx2& c, float* ap, const F4& s
         }
     } else {
         F4 a = ld4(ap);
-        const float w = (c.algo == PRL_ALGO_LINEAR) ? (float)(c.iter + 1) : 1.0f;  // LinearCFR.py:56-61
+        const float w = (c.algo == PRL_ALGO_LINEAR) ? (float)(c.iter + 1)                  // LinearCFR.py:56-61
+                        : (c.algo == PRL_ALGO_DCFR) ? c.B.dcfr[3 * (size_t)c.iter + 2] : 1.0f;
 #pragma unroll
         for (int i = 0; i < 4; ++i) a.v[i] = a.v[i] + r.v[i] * w;  // VanillaCFR.py:57-62
         st4(ap, a);
@@ -218,7 +236,7 @@ __device__ __forceinline__ F4 own_node_update(const Ctx2& c, int fs, int h0, con
 #pragma unroll
         for (int i = 0; i < 4; ++i) v.v[i] += s.v[i] * e[k].v[i];
     }
-    const float w = (float)(c.iter + 1);
+    const RegretW w = regret_w(c);
     F4 ssum = splat(0.0f);
 #pragma unroll
     for (int k = 0; k < A; ++k) {
@@ -286,7 +304,7 @@ __device__ __forceinline__ void value_rows(const Ctx2& c, int n, int fc, int fs,
             if (UPDATE && p == c.upd_p) {  // any fan-out: rows re-read from L1 / L2
                 float* rcol = c.B.regret + (size_t)fs * ld + h0;
                 float* scol = c.B.strat + (size_t)fs * ld + h0;
-                const float w = (float)(c.iter + 1);
+                const RegretW w = regret_w(c);
                 F4 ssum = splat(0.0f);
                 for (int k = 0; k < A; ++k) {  // pass A: positive regret mass (new regrets are recomputed in pass B)
                     const F4 e = ld4(ecol + (size_t)k * ld), rg = ld4(rcol + (size_t)k * ld);
@@ -1108,6 +1126,10 @@ int value_pass(const prl_tree_t* tree, const prl_buffers_t* buf, int player_mask
     return prl::check(cudaGetLastError(), "prl_value_pass(two-card)");
 }
 
+int check_dcfr(const prl_buffers_t* buf, int algo) {
+    return (algo == PRL_ALGO_DCFR && !buf->dcfr) ? prl::fail("prl: DCFR needs the factor table buf->dcfr") : 0;
+}
+
 int root_exploitability(const prl_tree_t* tree, const prl_buffers_t* buf, float* out, cudaStream_t s) {
     root_exploitability2_kernel<<<1, 256, 0, s>>>(*tree, *buf, out);
     prl::count_launch();
@@ -1117,6 +1139,8 @@ int root_exploitability(const prl_tree_t* tree, const prl_buffers_t* buf, float*
 int cfr_sweep(const prl_tree_t* tree, const prl_buffers_t* buf, int algo, int p, int iter, int delay, const int* mode,
               int which, cudaStream_t s) {
     if (int e = check_tree2(tree)) return e;
+    if (p < 0 || p > 1 || algo < 0 || algo > 3) return prl::fail("prl_cfr_sweep(two-card): bad p / algo");
+    if (int e = check_dcfr(buf, algo)) return e;
     Ctx2 c{*tree, *buf, 0, 0, 1 << p, {mode[0], mode[1]}, algo, p, iter, delay, 0.0f, 1.0f};
     set_avg_weights(c);
     if (which & 1)
@@ -1139,6 +1163,7 @@ extern "C" int prl_value_levels(const prl_tree_t* tree, const prl_buffers_t* buf
     if (int e = check_tree2(tree)) return e;
     if (level_hi >= tree->n_levels || level_lo < 0 || level_hi < level_lo) return prl::fail("prl_value_levels: bad level range");
     if (with_br && algo >= 0) return prl::fail("prl_value_levels: the update sweep does not compute best responses");
+    if (int e = prl2::check_dcfr(buf, algo)) return e;
     Ctx2 c{*tree, *buf, 0, 0, player_mask, {strat_mode[0], strat_mode[1]}, algo < 0 ? 0 : algo, algo < 0 ? -1 : upd_p, iter, delay, 0.0f, 1.0f};
     if (int e = value_levels2(c, with_br != 0, algo >= 0, level_hi, level_lo, chance_phase, (cudaStream_t)stream)) return e;
     return prl::check(cudaGetLastError(), "prl_value_levels");
@@ -1171,6 +1196,7 @@ extern "C" int prl_reach_levels(const prl_tree_t* tree, const prl_buffers_t* buf
     if (!tree || tree->n_hole != 2) return prl::fail("prl_reach_levels: two-card trees only");
     if (int e = check_tree2(tree)) return e;
     if (level_lo < 0 || level_hi >= tree->n_levels || level_lo > level_hi) return prl::fail("prl_reach_levels: bad level range");
+    if (int e = prl2::check_dcfr(buf, algo)) return e;
     Ctx2 c{*tree, *buf, 0, 0, player_mask, {strat_mode[0], strat_mode[1]}, algo < 0 ? 0 : algo, algo < 0 ? -1 : upd_p, iter, delay, 0.0f, 1.0f};
     set_avg_weights(c);
     const prl_tree_t& T = c.T;

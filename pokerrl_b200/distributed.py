@@ -15,6 +15,7 @@ import torch
 import torch.distributed as dist
 
 from pokerrl_b200 import _native as nat
+from pokerrl_b200 import dcfr as _dcfr
 from pokerrl_b200.game.flat_tree import FlatTree
 from pokerrl_b200.game.holdem_boards import BoardSpec
 from pokerrl_b200.solver import CFRSolver, TreeBuffers, TreeOps, _on, _stream
@@ -51,7 +52,7 @@ class ShardedCFRSolver(CFRSolver):
     world == 1 (or no process group) runs the same split schedule without communication."""
 
     def __init__(self, game_cls, env_args, board_spec, algo="CFRPlus", delay=0, device=None, rank=0, world=1,
-                 group=None, root_actions=None):
+                 group=None, root_actions=None, dcfr=_dcfr.DEFAULT):
         self.rank, self.world, self.group = rank, world, group
         ft = FlatTree(game_cls, env_args, board_spec=shard_board_spec(board_spec, rank, world) if world > 1 else board_spec,
                       root_actions=root_actions)
@@ -59,7 +60,7 @@ class ShardedCFRSolver(CFRSolver):
         if world > 1 and (ft.kind == nat.KIND_SHOWDOWN_ALLIN).any():
             raise NotImplementedError("all-in showdowns before the board is complete run out over ALL boards below them: "
                                       "not available with the boards sharded over ranks (run this tree on one GPU)")
-        super().__init__(ft, algo=algo, delay=delay, device=device, avg_f64=False, persistent=False)
+        super().__init__(ft, algo=algo, delay=delay, device=device, avg_f64=False, persistent=False, dcfr=dcfr)
         # levels holding BOUNDARY chance nodes: chance nodes right below the replicated trunk (no deal above them), whose
         # children - the boards of the first chance layer - are spread over the ranks.  Deeper chance nodes are local.
         self._n_chance, self._n_boundary = {}, {}
@@ -119,6 +120,7 @@ class ShardedCFRSolver(CFRSolver):
             self._iteration_sharded(n)
 
     def _iteration_sharded(self, n):
+        self._bind_factors(n)
         tree, buf = C.byref(self.dtree.desc), C.byref(self.bufs.desc)
         for _ in range(n):
             for p in (0, 1):

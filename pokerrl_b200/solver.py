@@ -11,8 +11,9 @@ import numpy as np
 import torch
 
 from pokerrl_b200 import _native as nat
+from pokerrl_b200 import dcfr as _dcfr
 
-ALGOS = {"VanillaCFR": nat.ALGO_VANILLA, "CFRPlus": nat.ALGO_CFR_PLUS, "LinearCFR": nat.ALGO_LINEAR}
+ALGOS = {"VanillaCFR": nat.ALGO_VANILLA, "CFRPlus": nat.ALGO_CFR_PLUS, "LinearCFR": nat.ALGO_LINEAR, "DCFR": nat.ALGO_DCFR}
 
 
 def _require_cuda(device):
@@ -320,14 +321,17 @@ class CFRSolver:
     strategy is a separate, optional evaluation (the reference does both every iteration).
     """
 
-    def __init__(self, ft, algo="CFRPlus", delay=0, device=None, avg_f64=False, persistent=True):
+    def __init__(self, ft, algo="CFRPlus", delay=0, device=None, avg_f64=False, persistent=True, dcfr=_dcfr.DEFAULT):
         self.persistent = bool(persistent)  # one cooperative launch per call instead of one launch per tree level
         self.ft = ft
         self.algo_name = algo
         self.algo = ALGOS[algo]
         self.delay = int(delay) if algo == "CFRPlus" else 0
         self.avg_f64 = bool(avg_f64) and algo == "CFRPlus"
+        # DCFR's (alpha, beta, gamma) and the device table of its per-iteration factors (None for the other algorithms)
+        self.dcfr = _dcfr.check_params(*dcfr) if algo == "DCFR" else None
         self.dtree = DeviceTree(ft, device)
+        self._factors = _dcfr.FactorTable(self.dcfr, self.dtree.device) if self.dcfr else None
         self.bufs = TreeBuffers(self.dtree, avg_dtype=torch.float64 if self.avg_f64 else torch.float32)
         self.ops = TreeOps(self.dtree, self.bufs)
         self._eval_bufs = None
@@ -345,7 +349,13 @@ class CFRSolver:
         with _on(self.dtree.device):
             self._iteration(n)
 
+    def _bind_factors(self, n):
+        """DCFR: the factor table covers the next n iterations"""
+        if self._factors is not None:
+            self.bufs.desc.dcfr = self._factors.ensure(self.iter_counter + n)
+
     def _iteration(self, n):
+        self._bind_factors(n)
         tree, buf = C.byref(self.dtree.desc), C.byref(self.bufs.desc)
         _stream = lambda: C.c_void_p(torch.cuda.current_stream(self.dtree.device).cuda_stream)  # noqa: E731
         if self.persistent and n > 0:
@@ -365,13 +375,13 @@ class CFRSolver:
     #      a no-op skeleton) - SURVEY.md §8f N1
     def state_dict(self):
         return {"engine": "levels", "algo": self.algo_name, "delay": self.delay, "avg_f64": self.avg_f64,
-                "rank": getattr(self, "rank", 0), "world": getattr(self, "world", 1), "n_nodes": self.ft.n_nodes,
+                "dcfr": list(self.dcfr) if self.dcfr else None, "rank": getattr(self, "rank", 0), "world": getattr(self, "world", 1), "n_nodes": self.ft.n_nodes,
                 "iter_counter": self.iter_counter, "modes": list(self.modes),
                 "regret": self.bufs.regret.cpu(), "strat": self.bufs.strat.cpu(), "avg": self.bufs.avg.cpu()}
 
     def load_state_dict(self, state):
         mine = {"engine": "levels", "algo": self.algo_name, "delay": self.delay, "avg_f64": self.avg_f64,
-                "rank": getattr(self, "rank", 0), "world": getattr(self, "world", 1), "n_nodes": self.ft.n_nodes}
+                "dcfr": list(self.dcfr) if self.dcfr else None, "rank": getattr(self, "rank", 0), "world": getattr(self, "world", 1), "n_nodes": self.ft.n_nodes}
         for k, v in mine.items():
             if state.get(k, v) != v:
                 raise ValueError("checkpoint mismatch on %r: file has %r, this solver %r" % (k, state.get(k), v))
