@@ -17,13 +17,13 @@ import numpy as np
 import torch
 
 from pokerrl_b200 import _native as nat
+from pokerrl_b200 import algorithm
 from pokerrl_b200 import dcfr as _dcfr
 from pokerrl_b200.game.flat_tree import FlatTree
 from pokerrl_b200.game.holdem_boards import BoardSpec
 from pokerrl_b200.solver import DeviceTree, TreeBuffers, TreeOps, _require_cuda
 
 SRC_REGRET, SRC_AVG, SRC_AVG_SUM = 0, 1, 2
-ALGOS = {"VanillaCFR": nat.ALGO_VANILLA, "CFRPlus": nat.ALGO_CFR_PLUS, "LinearCFR": nat.ALGO_LINEAR, "DCFR": nat.ALGO_DCFR}
 
 
 def board_layout(g=None):
@@ -41,7 +41,7 @@ def _stream(dev):
 def supports(game_cls, env_args, algo):
     """True iff the game's abstract tree is one pre-deal trunk + one chance layer + a compiled post-deal shape (Flop5Holdem:
     stacks of 301 chips and more; at 300 and below the preflop raise is all-in and there is no post-deal betting)"""
-    if algo not in ALGOS or game_cls.RULES.N_HOLE_CARDS != 2 or game_cls.RULES.N_CARDS_IN_DECK != 52:
+    if algo not in algorithm.ALGOS or game_cls.RULES.N_HOLE_CARDS != 2 or game_cls.RULES.N_CARDS_IN_DECK != 52:
         return False
     if game_cls.RULES.N_FLOP_CARDS != 5 or os.environ.get("PRL_ENGINE", "board") != "board":
         return False
@@ -272,16 +272,13 @@ class _BoardEngine:
 class BoardCFRSolver(_BoardEngine):
     def __init__(self, game_cls, env_args, board_spec=None, algo="CFRPlus", delay=0, device=None, rank=0, world=1,
                  group=None, grid=0, reduce_fn=None, dcfr=_dcfr.DEFAULT):
-        if algo not in ALGOS:
-            raise ValueError("unknown algorithm %r" % (algo,))
-        self.dcfr = _dcfr.check_params(*dcfr) if algo == "DCFR" else None
         self.device = _require_cuda(device)
-        self._factors = _dcfr.FactorTable(self.dcfr, self.device) if self.dcfr else None
+        self.alg = algorithm.Algorithm(algo, delay, dcfr, self.device)
+        self.algo_name, self.algo, self.delay, self.dcfr = self.alg.name, self.alg.code, self.alg.delay, self.alg.dcfr
+        self._factors = self.alg.factors  # DCFR's device table (None for the other algorithms), grown by factor_table
         self.rank, self.world, self.group = int(rank), int(world), group
         # cross-rank sum of the fixed-point chance sums, in place; default: torch.distributed all-reduce when world > 1
         self._reduce_fn = reduce_fn
-        self.algo_name, self.algo = algo, ALGOS[algo]
-        self.delay = int(delay) if algo == "CFRPlus" else 0
         self.game_cls, self.env_args = game_cls, env_args
         spec = board_spec if board_spec is not None else BoardSpec.full_game(game_cls.RULES)
         self.spec_full = spec
@@ -428,6 +425,7 @@ class BoardCFRSolver(_BoardEngine):
     def _update_begin(self, p):
         """first half of seat p's half-iteration: the board sweep (level path: the chance level's trunk terminals first)"""
         cl = self.chance_level
+        self.g.dcfr = self.alg.factor_table(self.iter_counter + 1)  # DCFR: read by this update's sweep and trunk
         if not self.fused_trunk:
             self._levels(self.bufs, 1 << p, False, self.algo, p, self.modes, cl, cl, 1)
         self._sweep_begin(self.bufs, p, False, SRC_REGRET, SRC_REGRET)
@@ -438,10 +436,7 @@ class BoardCFRSolver(_BoardEngine):
         if self.algo != nat.ALGO_CFR_PLUS:  # VanillaCFR.py:56-59 / LinearCFR.py:55-58: weight of this update's strategy in the sums
             if not self.fused_trunk:
                 raise RuntimeError("Vanilla / Linear CFR and DCFR on the board engine need the fused trunk (unset PRL_TRUNK=levels)")
-            if self.algo == nat.ALGO_DCFR:  # w_t of THIS iteration, whichever later sweep adds the contribution
-                self._pending[p] = self._factors.w(self.iter_counter)
-            else:
-                self._pending[p] = float(self.iter_counter + 1) if self.algo == nat.ALGO_LINEAR else 1.0
+            self._pending[p] = self.alg.sum_weight(self.iter_counter)  # THIS iteration's, whichever later sweep adds it
         if self.fused_trunk:
             self._reduce(self.w_total[:1])
             self._trunk(self.bufs, self.modes, False, p)
@@ -467,8 +462,6 @@ class BoardCFRSolver(_BoardEngine):
 
     def iteration(self, n=1):
         with torch.cuda.device(self.device):
-            if self._factors is not None:  # DCFR: the factor table covers the next n iterations
-                self.g.dcfr = self._factors.ensure(self.iter_counter + n)
             for _ in range(n):
                 for p in (0, 1):  # _CFRBase.py:122-128
                     self._update_begin(p)
@@ -484,36 +477,33 @@ class BoardCFRSolver(_BoardEngine):
             self._trunk(bufs, modes, True, -1)
             self._next_generation()
             e = self._expl.cpu().numpy()
-            return sum(float(e[p]) * self.ev_normalizer for p in range(2)) / 2
-        self._levels(bufs, 3, True, -1, -1, modes, cl, cl, 1)
-        for p in (0, 1):
-            self._sweep(bufs, p, True, src, src)
-        self._levels(bufs, 3, True, -1, -1, modes, cl, cl, 2)
-        if cl > 0:
-            self._levels(bufs, 3, True, -1, -1, modes, cl - 1, 0, 0)
-        ops = TreeOps(self.trunk, bufs) if bufs is not self.bufs else self.ops
-        e = ops.root_exploitability()
-        return sum(float(e[p]) * self.ev_normalizer for p in range(2)) / 2
+        else:
+            self._levels(bufs, 3, True, -1, -1, modes, cl, cl, 1)
+            for p in (0, 1):
+                self._sweep(bufs, p, True, src, src)
+            self._levels(bufs, 3, True, -1, -1, modes, cl, cl, 2)
+            if cl > 0:
+                self._levels(bufs, 3, True, -1, -1, modes, cl - 1, 0, 0)
+            e = (TreeOps(self.trunk, bufs) if bufs is not self.bufs else self.ops).root_exploitability()
+        return algorithm.seat_averaged(e, self.ev_normalizer)
 
     def exploitability_current(self):
         with torch.cuda.device(self.device):
             return self._evaluate(self.bufs, self.modes, SRC_REGRET)
 
     def exploitability_average(self):
-        if self.iter_counter <= self.delay:
-            raise RuntimeError("no average strategy before iteration delay+1 (CFRPlus.py:33-35)")
+        # the board engine has no average before the first iteration for any algorithm; the level engine evaluates the
+        # still-empty sums of Vanilla / Linear CFR and DCFR as the uniform strategy
+        if self.iter_counter == 0:
+            raise RuntimeError("no average strategy before the first iteration")
+        m, src = {algorithm.SUMS: (nat.STRAT_AVG_SUM, SRC_AVG_SUM), algorithm.CURRENT: (nat.STRAT_F32, SRC_REGRET),
+                  algorithm.AVERAGE: (nat.STRAT_AVG_F32, SRC_AVG)}[self.alg.average(self.iter_counter)]
         with torch.cuda.device(self.device):
             if self._eval_bufs is None:
                 self._eval_bufs = TreeBuffers(self.trunk, share=self.bufs)
             self.flush_average()
-            if self.algo != nat.ALGO_CFR_PLUS:  # normalised reach-weighted sums (LinearCFR.py:64-71, VanillaCFR.py:65-72)
-                modes, src = [nat.STRAT_AVG_SUM, nat.STRAT_AVG_SUM], SRC_AVG_SUM
-            elif self.iter_counter == self.delay + 1:  # avg == copy of the current strategy (CFRPlus.py:83-84)
-                modes, src = [nat.STRAT_F32, nat.STRAT_F32], SRC_REGRET
-            else:
-                modes, src = [nat.STRAT_AVG_F32, nat.STRAT_AVG_F32], SRC_AVG
-            self._reach_trunk(self._eval_bufs, 3, -1, -1, modes, self.iter_counter, self.delay)
-            return self._evaluate(self._eval_bufs, modes, src)
+            self._reach_trunk(self._eval_bufs, 3, -1, -1, [m, m], self.iter_counter, self.delay)
+            return self._evaluate(self._eval_bufs, [m, m], src)
 
     # ------------------------------------------------------------------------------------------------ interfaces
     def natural_tables(self, ft):
@@ -553,20 +543,18 @@ class BoardCFRSolver(_BoardEngine):
         with torch.cuda.device(self.device):
             self._reach_trunk(self.bufs, 3, -1, -1, self.modes, self.iter_counter, self.delay)
 
+    def _identity(self):
+        return {"engine": "board", **self.alg.identity(), "rank": self.rank, "world": self.world, "n_boards": self.n_boards,
+                "n_boards_total": self.n_boards_total}
+
     def state_dict(self):
         self.flush_average()
-        return {"engine": "board", "algo": self.algo_name, "delay": self.delay, "dcfr": list(self.dcfr) if self.dcfr else None,
-                "iter_counter": self.iter_counter,
-                "modes": list(self.modes), "rank": self.rank, "world": self.world, "n_boards": self.n_boards,
-                "n_boards_total": self.n_boards_total, "regret": self.regret.cpu(), "avg": self.avg.cpu(),
+        return {**self._identity(), "iter_counter": self.iter_counter, "modes": list(self.modes),
+                "regret": self.regret.cpu(), "avg": self.avg.cpu(),
                 "trunk_regret": self.bufs.regret.cpu(), "trunk_strat": self.bufs.strat.cpu(), "trunk_avg": self.bufs.avg.cpu()}
 
     def load_state_dict(self, state):
-        for k in ("engine", "algo", "delay", "dcfr", "rank", "world", "n_boards", "n_boards_total"):
-            mine = {"engine": "board", "algo": self.algo_name, "dcfr": list(self.dcfr) if self.dcfr else None}.get(
-                k, getattr(self, k, None))
-            if state.get(k) != mine:
-                raise ValueError("checkpoint mismatch on %r: file has %r, this solver %r" % (k, state.get(k), mine))
+        algorithm.check_identity(state, self._identity())
         if tuple(state["regret"].shape) != tuple(self.regret.shape):
             raise ValueError("checkpoint table shape %s != %s" % (tuple(state["regret"].shape), tuple(self.regret.shape)))
         self.iter_counter, self.modes = int(state["iter_counter"]), list(state["modes"])
@@ -737,17 +725,15 @@ class BoardPolicyTables:
         if s.world != 1:
             raise ValueError("a sharded solver holds only its rank's boards")
         s.flush_average()
-        cfrp = s.algo == nat.ALGO_CFR_PLUS
-        if cfrp and s.iter_counter <= s.delay:
-            raise RuntimeError("CFR+ has no average strategy before iteration delay+1")
+        avg = s.alg.average(s.iter_counter)
         nb, rpb, st = s.n_boards, s.rows_per_board, s.st
         groups = [[s.local_rows[c][0] for c in range(st["first_child"][d], st["first_child"][d] + st["n_children"][d])]
                   for d in _decision_locals(st)]
         with torch.cuda.device(s.device):
-            if cfrp and s.iter_counter > s.delay + 1:
+            if avg == algorithm.AVERAGE:
                 rows = s.avg.clone()
             else:
-                matching = cfrp  # regret matching at delay + 1, else normalised sums
+                matching = avg == algorithm.CURRENT  # regret matching at delay + 1, else normalised sums
                 rows = torch.empty_like(s.avg)
                 src = (s.regret if matching else s.avg).view(nb, rpb, -1)
                 dst = rows.view(nb, rpb, -1)
@@ -756,8 +742,8 @@ class BoardPolicyTables:
                     for idx in groups:
                         dst[lo:hi, idx] = _normalised(src[lo:hi, idx], 1, matching)
             nts, ft = s.n_trunk_slots, s.ft1
-            if cfrp:
-                trunk = (s.bufs.strat if s.iter_counter == s.delay + 1 else s.bufs.avg)[:nts].clone()
+            if avg != algorithm.SUMS:
+                trunk = (s.bufs.strat if avg == algorithm.CURRENT else s.bufs.avg)[:nts].clone()
             else:
                 a = s.bufs.avg[:nts]
                 trunk = torch.zeros_like(a)

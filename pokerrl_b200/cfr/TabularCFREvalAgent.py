@@ -9,7 +9,7 @@ game) and answers for any Flop5Holdem PublicTree - any board spec, either engine
 (prl_board_policy_query)."""
 import numpy as np
 
-from pokerrl_b200 import _native as nat
+from pokerrl_b200 import algorithm
 from pokerrl_b200.rl.base_cls.EvalAgentBase import EvalAgentBase
 
 
@@ -25,10 +25,9 @@ def tree_fingerprint(ft):
 def average_strategy_table(solver):
     """float32 [n_slots, R] average strategy of a CFRSolver (host copy), normalised like the reference's `avg_strat`."""
     ft, R = solver.ft, solver.ft.R
-    if solver.algo == nat.ALGO_CFR_PLUS:
-        if solver.iter_counter <= solver.delay:
-            raise RuntimeError("CFR+ has no average strategy before iteration delay+1")
-        src = solver.bufs.strat if solver.iter_counter == solver.delay + 1 else solver.bufs.avg
+    avg = solver.alg.average(solver.iter_counter)
+    if avg != algorithm.SUMS:
+        src = solver.bufs.strat if avg == algorithm.CURRENT else solver.bufs.avg
         return src[:, :R].float().cpu().numpy()
     s = solver.bufs.avg[:, :R].cpu().numpy()
     out = np.empty_like(s)

@@ -1270,14 +1270,6 @@ int launch_sweep(const SweepArgs& a, int grid, cudaStream_t s) {
     return 0;
 }
 
-// CFRPlus.py:68-73: weights of the averaging step of iteration iter (the first one, iter == delay, copies the strategy)
-void cfrp_weights(int iter, int delay, float* m_old, float* m_new) {
-    const double cw = 0.5 * ((double)iter * (iter + 1) - (double)delay * (delay + 1));
-    const double nw = (double)iter - delay + 1;
-    *m_old = (iter > delay) ? (float)(cw / (cw + nw)) : 0.0f;
-    *m_new = (iter > delay) ? (float)(nw / (cw + nw)) : 1.0f;
-}
-
 }  // namespace
 
 extern "C" int prl_board_layout(const prl_board_game_t* shape, int32_t* out) {
@@ -1325,9 +1317,7 @@ extern "C" int prl_board_build_tables(const int32_t* ranks, const uint64_t* boar
 // written, 0: it is left pending.  Today's form (-1, 1), deferred (-1, 0), paired (due, 1).
 static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, int src_opp, const float* trunk_reach_opp, int iter,
                        int delay, int algo, float defer_w, int p1_only, int due, int now, prl_stream_t stream) {
-    if (algo < PRL_ALGO_VANILLA || algo > PRL_ALGO_DCFR) return prl::fail("prl_board_sweep: bad algo");
-    if (algo == PRL_ALGO_DCFR && !eval && !p1_only && !g->dcfr)
-        return prl::fail("prl_board_sweep: DCFR needs the factor table g->dcfr");
+    if (int e = prl::check_algo(algo, g->dcfr, !eval && !p1_only, "prl_board_sweep")) return e;
     const bool defer = !eval && algo != PRL_ALGO_CFR_PLUS;
     if (p1_only && !defer) return prl::fail("prl_board_sweep: p1_only is the average flush of Vanilla / Linear CFR");
     const int layout_ok = with_shape(g, [&](auto sh) { return layout_matches<decltype(sh)>(g) ? 1 : 0; });
@@ -1347,14 +1337,14 @@ static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, 
     a.trunk_reach_opp = trunk_reach_opp;
     a.iter = iter;
     a.delay = delay;
-    cfrp_weights(iter, delay, &a.m_old, &a.m_new);
+    prl::cfrp_weights(iter, delay, &a.m_old, &a.m_new);
     a.pair = due >= 0;
     a.m_old_due = a.m_new_due = 0.0f;
-    if (a.pair) cfrp_weights(due, delay, &a.m_old_due, &a.m_new_due);
+    if (a.pair) prl::cfrp_weights(due, delay, &a.m_old_due, &a.m_new_due);
     a.src_own = src_own;
     a.src_opp = src_opp;
-    a.rw = (algo == PRL_ALGO_LINEAR) ? (float)(iter + 1) : 1.0f;
-    a.disc = (algo == PRL_ALGO_DCFR && !eval && !p1_only) ? g->dcfr + 3 * (size_t)iter : nullptr;
+    a.rw = prl::regret_weight(algo, iter);
+    a.disc = prl::dcfr_row(algo, g->dcfr, iter, !eval && !p1_only);
     a.defer_w = defer ? defer_w : 0.0f;
     a.fx_scale = (double)(1ull << g->frac_bits);
     for (int n = 0; n < 16; ++n) {
@@ -1402,7 +1392,7 @@ extern "C" int prl_board_avg_flush(const prl_board_game_t* g, int p, int due, in
     if (!g->regret || !g->avg) return prl::fail("prl_board_avg_flush: missing buffers");
     if (g->n_boards <= 0) return 0;
     float m_old, m_new;
-    cfrp_weights(due, delay, &m_old, &m_new);
+    prl::cfrp_weights(due, delay, &m_old, &m_new);
     cudaStream_t s = (cudaStream_t)stream;
     with_shape(g, [&](auto sh) {
         using SH = decltype(sh);
@@ -1475,11 +1465,10 @@ extern "C" int prl_board_policy_query(const prl_board_game_t* shape, const float
 extern "C" int prl_board_trunk(const prl_board_game_t* g, const prl_trunk_t* t, int eval, int p, int n_sym, const int16_t* sym_perm,
                                int iter, int delay, float* out_expl, const int64_t* const* peers, int n_peers,
                                int64_t peer_offset, int64_t* w_scratch, int algo, prl_stream_t stream) {
-    if (algo < PRL_ALGO_VANILLA || algo > PRL_ALGO_DCFR) return prl::fail("prl_board_trunk: bad algo");
-    if (algo == PRL_ALGO_DCFR && !eval && (!g || !g->dcfr)) return prl::fail("prl_board_trunk: DCFR needs the factor table g->dcfr");
-    const float rw = (algo == PRL_ALGO_LINEAR) ? (float)(iter + 1) : 1.0f;
-    const float* disc = (algo == PRL_ALGO_DCFR && !eval) ? g->dcfr + 3 * (size_t)iter : nullptr;
+    if (int e = prl::check_algo(algo, g ? g->dcfr : nullptr, !eval, "prl_board_trunk")) return e;
     if (!g || !t || t->n_nodes < 1 || t->n_nodes > 8) return prl::fail("prl_board_trunk: 1..8 trunk nodes");
+    const float rw = prl::regret_weight(algo, iter);
+    const float* disc = prl::dcfr_row(algo, g->dcfr, iter, !eval);
     if (with_shape(g, [](auto) { return 0; }) == kNoShape) return prl::fail("prl_board_trunk: the post-deal subtree has no compiled shape");
     if (t->n_range != kRange || g->n_deck != kDeck) return prl::fail("prl_board_trunk: 52-card deck / 1326 hands only");
     if (eval && !out_expl) return prl::fail("prl_board_trunk: out_expl missing");
@@ -1487,7 +1476,7 @@ extern "C" int prl_board_trunk(const prl_board_game_t* g, const prl_trunk_t* t, 
         if (t->kind[n] == PRL_KIND_SHOWDOWN || t->kind[n] == PRL_KIND_SHOWDOWN_ALLIN)
             return prl::fail("prl_board_trunk: showdowns before the deal are not supported");
     float m_old, m_new;
-    cfrp_weights(iter, delay, &m_old, &m_new);
+    prl::cfrp_weights(iter, delay, &m_old, &m_new);
     const double inv_scale = 1.0 / (double)(1ull << g->frac_bits);
     const long long* w = reinterpret_cast<const long long*>(g->w_total);
     if (peers && (n_peers < 1 || !w_scratch)) return prl::fail("prl_board_trunk: peer sum needs n_peers >= 1 and w_scratch");

@@ -310,29 +310,6 @@ __device__ __forceinline__ float fold_children(const float* __restrict__ col, in
     return v;
 }
 
-// weights of the regret update of iteration c.iter: Linear CFR's iter + 1, DCFR's discounts of positive / negative sums
-struct RegretW {
-    float w, a, b;
-};
-__device__ __forceinline__ RegretW regret_w(const Ctx& c) {
-    RegretW r{(float)(c.iter + 1), 1.0f, 1.0f};
-    if (c.algo == PRL_ALGO_DCFR) {
-        r.a = c.B.dcfr[3 * (size_t)c.iter];
-        r.b = c.B.dcfr[3 * (size_t)c.iter + 1];
-    }
-    return r;
-}
-
-__device__ __forceinline__ float regret_step(int algo, float d, float old, const RegretW& w) {
-    if (algo == PRL_ALGO_CFR_PLUS) return fmaxf(d + old, 0.0f);  // CFRPlus.py:37-41
-    if (algo == PRL_ALGO_LINEAR) return w.w * d + old;           // LinearCFR.py:27-31
-    if (algo == PRL_ALGO_DCFR) {                                 // discounted after this iteration's regret is added
-        const float x = d + old;
-        return x * ((x > 0.0f) ? w.a : w.b);
-    }
-    return d + old;                                              // VanillaCFR.py:26-30
-}
-
 // Seat p acts at this node and is being updated, A children (compile time): node value with the current strategy,
 // regret update (_CFRBase.py:146-185) and regret matching (CFRPlus.py:43-63 and siblings).  Everything the lane needs
 // is requested before the first use; returns the node value.
@@ -361,11 +338,11 @@ __device__ __forceinline__ float update_own(const Ctx& c, int md, const float* _
         for (int k = 1; k < A; ++k) acc = acc + strat_f64(c, md, fs, k, A, h) * (double)e[k];
         v = (float)acc;
     }
-    const RegretW w = regret_w(c);
+    const prl::RegretW w = prl::regret_w(c);
     float ssum = 0.0f;
 #pragma unroll
     for (int k = 0; k < A; ++k) {
-        rg[k] = regret_step(c.algo, e[k] - v, rg[k], w);
+        rg[k] = prl::regret_step(c.algo, e[k] - v, rg[k], w);
         const float rp = fmaxf(rg[k], 0.0f);
         ssum = (k == 0) ? rp : ssum + rp;
     }
@@ -454,16 +431,16 @@ __device__ __forceinline__ void value_group(const Ctx& c, const int lo, const in
                 if (upd) {  // wide node: stream (regrets are recomputed in the second loop instead of re-read)
                     float* rcol = c.B.regret + (size_t)fs * ld + h;
                     float* scol = c.B.strat + (size_t)fs * ld + h;
-                    const RegretW w = regret_w(c);
+                    const prl::RegretW w = prl::regret_w(c);
                     float ssum = 0.0f;
                     for (int k = 0; k < A; ++k) {
-                        const float rp = fmaxf(regret_step(c.algo, ecol[(size_t)k * ld] - v, rcol[(size_t)k * ld], w), 0.0f);
+                        const float rp = fmaxf(prl::regret_step(c.algo, ecol[(size_t)k * ld] - v, rcol[(size_t)k * ld], w), 0.0f);
                         ssum = (k == 0) ? rp : ssum + rp;
                     }
                     const float uni = (float)(1.0 / (double)A);
                     const float den = (ssum > 0.0f) ? ssum : 1.0f;
                     for (int k = 0; k < A; ++k) {
-                        const float r = regret_step(c.algo, ecol[(size_t)k * ld] - v, rcol[(size_t)k * ld], w);
+                        const float r = prl::regret_step(c.algo, ecol[(size_t)k * ld] - v, rcol[(size_t)k * ld], w);
                         rcol[(size_t)k * ld] = r;
                         const float q = fmaxf(r, 0.0f) / den;
                         scol[(size_t)k * ld] = (ssum > 0.0f) ? q : uni;
@@ -689,8 +666,8 @@ extern "C" int prl_cfr_sweep(const prl_tree_t* tree, const prl_buffers_t* buf, i
         return prl2::cfr_sweep(tree, buf, algo, p, iter, delay, strat_mode, which, (cudaStream_t)stream);
     }
     if (int e = check_tree(tree)) return e;
-    if (p < 0 || p > 1 || algo < 0 || algo > 3) return prl::fail("prl_cfr_sweep: bad p / algo");
-    if (algo == PRL_ALGO_DCFR && !buf->dcfr) return prl::fail("prl_cfr_sweep: DCFR needs the factor table buf->dcfr");
+    if (p < 0 || p > 1) return prl::fail("prl_cfr_sweep: bad p");
+    if (int e = prl::check_algo(algo, buf->dcfr, true, "prl_cfr_sweep")) return e;
     if (algo != PRL_ALGO_CFR_PLUS && avg_f64) return prl::fail("avg_f64 only applies to CFR+");
     Ctx c{*tree, *buf, 0, 0, 1 << p, {strat_mode[0], strat_mode[1]}, algo, p, iter, delay, avg_f64};
     if (which & 1) value_sweep(c, false, true, (cudaStream_t)stream);
@@ -768,8 +745,8 @@ extern "C" int prl_cfr_iterations(const prl_tree_t* tree, const prl_buffers_t* b
         return 0;
     }
     if (int e = check_tree(tree)) return e;
-    if (algo < 0 || algo > 3 || n_iters < 0) return prl::fail("prl_cfr_iterations: bad algo / n_iters");
-    if (algo == PRL_ALGO_DCFR && !buf->dcfr) return prl::fail("prl_cfr_iterations: DCFR needs the factor table buf->dcfr");
+    if (n_iters < 0) return prl::fail("prl_cfr_iterations: bad n_iters");
+    if (int e = prl::check_algo(algo, buf->dcfr, true, "prl_cfr_iterations")) return e;
     if (algo != PRL_ALGO_CFR_PLUS && avg_f64) return prl::fail("avg_f64 only applies to CFR+");
     if (n_iters == 0) return 0;
     Ctx c{*tree, *buf, 0, 0, 0, {strat_mode[0], strat_mode[1]}, algo, 0, iter0, delay, avg_f64};

@@ -88,30 +88,6 @@ __device__ __forceinline__ bool hand_blocked(const prl_tree_t& T, int h, unsigne
 }
 
 // ------------------------------------------------------------------------------------------------ CFR rules
-// weights of the regret update of iteration c.iter: Linear CFR's iter + 1, DCFR's discounts of positive / negative sums
-struct RegretW {
-    float w, a, b;
-};
-__device__ __forceinline__ RegretW regret_w(const Ctx2& c) {
-    RegretW r{(float)(c.iter + 1), 1.0f, 1.0f};
-    if (c.algo == PRL_ALGO_DCFR) {
-        r.a = c.B.dcfr[3 * (size_t)c.iter];
-        r.b = c.B.dcfr[3 * (size_t)c.iter + 1];
-    }
-    return r;
-}
-
-// new regret of one (row, hand) from the instantaneous regret d = v(child) - v(node) and the stored regret
-__device__ __forceinline__ float regret_step(int algo, float d, float old, const RegretW& w) {
-    if (algo == PRL_ALGO_CFR_PLUS) return fmaxf(d + old, 0.0f);
-    if (algo == PRL_ALGO_LINEAR) return w.w * d + old;
-    if (algo == PRL_ALGO_DCFR) {  // discounted after this iteration's regret is added
-        const float x = d + old;
-        return x * ((x > 0.0f) ? w.a : w.b);
-    }
-    return d + old;
-}
-
 // regret matching of one node's rows: a row's positive regret over the node's positive regret mass, uniform where that
 // mass is 0
 struct RegretMatch {
@@ -236,13 +212,13 @@ __device__ __forceinline__ F4 own_node_update(const Ctx2& c, int fs, int h0, con
 #pragma unroll
         for (int i = 0; i < 4; ++i) v.v[i] += s.v[i] * e[k].v[i];
     }
-    const RegretW w = regret_w(c);
+    const prl::RegretW w = prl::regret_w(c);
     F4 ssum = splat(0.0f);
 #pragma unroll
     for (int k = 0; k < A; ++k) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-            rg[k].v[i] = regret_step(c.algo, e[k].v[i] - v.v[i], rg[k].v[i], w);
+            rg[k].v[i] = prl::regret_step(c.algo, e[k].v[i] - v.v[i], rg[k].v[i], w);
             ssum.v[i] += fmaxf(rg[k].v[i], 0.0f);
         }
     }
@@ -304,19 +280,19 @@ __device__ __forceinline__ void value_rows(const Ctx2& c, int n, int fc, int fs,
             if (UPDATE && p == c.upd_p) {  // any fan-out: rows re-read from L1 / L2
                 float* rcol = c.B.regret + (size_t)fs * ld + h0;
                 float* scol = c.B.strat + (size_t)fs * ld + h0;
-                const RegretW w = regret_w(c);
+                const prl::RegretW w = prl::regret_w(c);
                 F4 ssum = splat(0.0f);
                 for (int k = 0; k < A; ++k) {  // pass A: positive regret mass (new regrets are recomputed in pass B)
                     const F4 e = ld4(ecol + (size_t)k * ld), rg = ld4(rcol + (size_t)k * ld);
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) ssum.v[i] += fmaxf(regret_step(c.algo, e.v[i] - v.v[i], rg.v[i], w), 0.0f);
+                    for (int i = 0; i < 4; ++i) ssum.v[i] += fmaxf(prl::regret_step(c.algo, e.v[i] - v.v[i], rg.v[i], w), 0.0f);
                 }
                 const RegretMatch rm(ssum, A);
                 for (int k = 0; k < A; ++k) {  // pass B: store regrets and the regret-matching strategy
                     const F4 e = ld4(ecol + (size_t)k * ld);
                     F4 rg = ld4(rcol + (size_t)k * ld);
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) rg.v[i] = regret_step(c.algo, e.v[i] - v.v[i], rg.v[i], w);
+                    for (int i = 0; i < 4; ++i) rg.v[i] = prl::regret_step(c.algo, e.v[i] - v.v[i], rg.v[i], w);
                     st4(rcol + (size_t)k * ld, rg);
                     st4(scol + (size_t)k * ld, rm(rg));
                 }
@@ -916,14 +892,6 @@ __global__ void root_exploitability2_kernel(prl_tree_t T, prl_buffers_t B, float
     }
 }
 
-// CFR+ linear averaging weights of iteration c.iter (CFRPlus.py:68-73)
-inline void set_avg_weights(Ctx2& c) {
-    const double cw = 0.5 * ((double)c.iter * (c.iter + 1) - (double)c.delay * (c.delay + 1));
-    const double nw = (double)c.iter - c.delay + 1;
-    c.m_old = (float)(cw / (cw + nw));
-    c.m_new = (float)(nw / (cw + nw));
-}
-
 inline unsigned blocks_for(long long threads) { return (unsigned)((threads + kThreads - 1) / kThreads); }
 
 int check_tree2(const prl_tree_t* t) {
@@ -1126,10 +1094,6 @@ int value_pass(const prl_tree_t* tree, const prl_buffers_t* buf, int player_mask
     return prl::check(cudaGetLastError(), "prl_value_pass(two-card)");
 }
 
-int check_dcfr(const prl_buffers_t* buf, int algo) {
-    return (algo == PRL_ALGO_DCFR && !buf->dcfr) ? prl::fail("prl: DCFR needs the factor table buf->dcfr") : 0;
-}
-
 int root_exploitability(const prl_tree_t* tree, const prl_buffers_t* buf, float* out, cudaStream_t s) {
     root_exploitability2_kernel<<<1, 256, 0, s>>>(*tree, *buf, out);
     prl::count_launch();
@@ -1139,10 +1103,10 @@ int root_exploitability(const prl_tree_t* tree, const prl_buffers_t* buf, float*
 int cfr_sweep(const prl_tree_t* tree, const prl_buffers_t* buf, int algo, int p, int iter, int delay, const int* mode,
               int which, cudaStream_t s) {
     if (int e = check_tree2(tree)) return e;
-    if (p < 0 || p > 1 || algo < 0 || algo > 3) return prl::fail("prl_cfr_sweep(two-card): bad p / algo");
-    if (int e = check_dcfr(buf, algo)) return e;
+    if (p < 0 || p > 1) return prl::fail("prl_cfr_sweep(two-card): bad p");
+    if (int e = prl::check_algo(algo, buf->dcfr, true, "prl_cfr_sweep(two-card)")) return e;
     Ctx2 c{*tree, *buf, 0, 0, 1 << p, {mode[0], mode[1]}, algo, p, iter, delay, 0.0f, 1.0f};
-    set_avg_weights(c);
+    prl::cfrp_weights(iter, delay, &c.m_old, &c.m_new);
     if (which & 1)
         if (int e = value_sweep2(c, false, true, s)) return e;
     if (which & 2) {
@@ -1163,7 +1127,8 @@ extern "C" int prl_value_levels(const prl_tree_t* tree, const prl_buffers_t* buf
     if (int e = check_tree2(tree)) return e;
     if (level_hi >= tree->n_levels || level_lo < 0 || level_hi < level_lo) return prl::fail("prl_value_levels: bad level range");
     if (with_br && algo >= 0) return prl::fail("prl_value_levels: the update sweep does not compute best responses");
-    if (int e = prl2::check_dcfr(buf, algo)) return e;
+    if (algo >= 0)
+        if (int e = prl::check_algo(algo, buf->dcfr, true, "prl_value_levels")) return e;
     Ctx2 c{*tree, *buf, 0, 0, player_mask, {strat_mode[0], strat_mode[1]}, algo < 0 ? 0 : algo, algo < 0 ? -1 : upd_p, iter, delay, 0.0f, 1.0f};
     if (int e = value_levels2(c, with_br != 0, algo >= 0, level_hi, level_lo, chance_phase, (cudaStream_t)stream)) return e;
     return prl::check(cudaGetLastError(), "prl_value_levels");
@@ -1196,9 +1161,10 @@ extern "C" int prl_reach_levels(const prl_tree_t* tree, const prl_buffers_t* buf
     if (!tree || tree->n_hole != 2) return prl::fail("prl_reach_levels: two-card trees only");
     if (int e = check_tree2(tree)) return e;
     if (level_lo < 0 || level_hi >= tree->n_levels || level_lo > level_hi) return prl::fail("prl_reach_levels: bad level range");
-    if (int e = prl2::check_dcfr(buf, algo)) return e;
+    if (algo >= 0)
+        if (int e = prl::check_algo(algo, buf->dcfr, true, "prl_reach_levels")) return e;
     Ctx2 c{*tree, *buf, 0, 0, player_mask, {strat_mode[0], strat_mode[1]}, algo < 0 ? 0 : algo, algo < 0 ? -1 : upd_p, iter, delay, 0.0f, 1.0f};
-    set_avg_weights(c);
+    prl::cfrp_weights(iter, delay, &c.m_old, &c.m_new);
     const prl_tree_t& T = c.T;
     for (int d = level_lo; d <= level_hi; ++d) {
         c.lo = (int)T.level_start[d];

@@ -1,4 +1,4 @@
-// Error reporting + ABI version for the pokerrl_b200 C ABI (include/pokerrl_b200.h).
+// Error reporting, ABI version and the algorithm check for the pokerrl_b200 C ABI (include/pokerrl_b200.h).
 #include <stdio.h>
 #include <string.h>
 
@@ -22,6 +22,14 @@ int check(cudaError_t e, const char* where) {
     return (int)e;
 }
 void count_launch() { ++g_launches; }
+
+int check_algo(int algo, const float* dcfr, bool updates, const char* where) {
+    char msg[256];
+    if (algo < PRL_ALGO_VANILLA || algo > PRL_ALGO_DCFR) snprintf(msg, sizeof(msg), "%s: bad algo %d", where, algo);
+    else if (updates && algo == PRL_ALGO_DCFR && !dcfr) snprintf(msg, sizeof(msg), "%s: DCFR needs the factor table dcfr", where);
+    else return 0;
+    return fail(msg);
+}
 }  // namespace prl
 
 extern "C" int prl_abi_version(void) { return PRL_ABI_VERSION; }

@@ -18,7 +18,7 @@ from pokerrl_b200 import _native as nat
 from pokerrl_b200 import dcfr as _dcfr
 from pokerrl_b200.game.flat_tree import FlatTree
 from pokerrl_b200.game.holdem_boards import BoardSpec
-from pokerrl_b200.solver import CFRSolver, TreeBuffers, TreeOps, _on, _stream
+from pokerrl_b200.solver import CFRSolver, _on, _stream
 
 
 def shard_board_spec(spec, rank, world):
@@ -72,11 +72,6 @@ class ShardedCFRSolver(CFRSolver):
                 self._n_boundary[d] = int((ch & (ft.cdepth[lo:hi] == 0)).sum())
         self._chance_levels = [d for d in self._n_chance if self._n_boundary[d] > 0]
         self.n_allreduce = 0
-        self._reach_stale = False
-
-    def reset(self):
-        super().reset()  # includes a full reach pass
-        self._reach_stale = False
 
     # ---- the one collective of the path
     def _allreduce_chance_sums(self, bufs, level, arrays):
@@ -129,23 +124,6 @@ class ShardedCFRSolver(CFRSolver):
                 nat.call("prl_reach_update", tree, buf, self.algo, p, self.iter_counter, self.delay, _stream())
             self.iter_counter += 1
 
-    def exploitability_current(self):
+    def _value_pass_br(self, ops, modes):
         with _on(self.dtree.device):
-            return self._exploitability_current()
-
-    def _exploitability_current(self):
-        if self._reach_stale:
-            self.ops.reach_pass(self.modes)
-            self._reach_stale = False
-        self._value_sweep(self.bufs, 3, True, -1, -1, self.modes)
-        return self._metric(self.ops.root_exploitability())
-
-    def exploitability_average(self):
-        with _on(self.dtree.device):
-            if self._eval_bufs is None:
-                self._eval_bufs = TreeBuffers(self.dtree, share=self.bufs)
-                self._eval_ops = TreeOps(self.dtree, self._eval_bufs)
-            m = self.average_modes()
-            self._eval_ops.reach_pass(m)
-            self._value_sweep(self._eval_bufs, 3, True, -1, -1, m)
-            return self._metric(self._eval_ops.root_exploitability())
+            self._value_sweep(ops.bufs, 3, True, -1, -1, modes)

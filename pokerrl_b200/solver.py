@@ -11,9 +11,8 @@ import numpy as np
 import torch
 
 from pokerrl_b200 import _native as nat
+from pokerrl_b200 import algorithm
 from pokerrl_b200 import dcfr as _dcfr
-
-ALGOS = {"VanillaCFR": nat.ALGO_VANILLA, "CFRPlus": nat.ALGO_CFR_PLUS, "LinearCFR": nat.ALGO_LINEAR, "DCFR": nat.ALGO_DCFR}
 
 
 def _require_cuda(device):
@@ -324,14 +323,11 @@ class CFRSolver:
     def __init__(self, ft, algo="CFRPlus", delay=0, device=None, avg_f64=False, persistent=True, dcfr=_dcfr.DEFAULT):
         self.persistent = bool(persistent)  # one cooperative launch per call instead of one launch per tree level
         self.ft = ft
-        self.algo_name = algo
-        self.algo = ALGOS[algo]
-        self.delay = int(delay) if algo == "CFRPlus" else 0
-        self.avg_f64 = bool(avg_f64) and algo == "CFRPlus"
-        # DCFR's (alpha, beta, gamma) and the device table of its per-iteration factors (None for the other algorithms)
-        self.dcfr = _dcfr.check_params(*dcfr) if algo == "DCFR" else None
+        self.alg = algorithm.Algorithm(algo, delay, dcfr, _require_cuda(device))
+        self.algo_name, self.algo, self.delay, self.dcfr = self.alg.name, self.alg.code, self.alg.delay, self.alg.dcfr
+        self._factors = self.alg.factors  # DCFR's device table (None for the other algorithms), grown by factor_table
+        self.avg_f64 = bool(avg_f64) and self.algo == nat.ALGO_CFR_PLUS
         self.dtree = DeviceTree(ft, device)
-        self._factors = _dcfr.FactorTable(self.dcfr, self.dtree.device) if self.dcfr else None
         self.bufs = TreeBuffers(self.dtree, avg_dtype=torch.float64 if self.avg_f64 else torch.float32)
         self.ops = TreeOps(self.dtree, self.bufs)
         self._eval_bufs = None
@@ -351,8 +347,7 @@ class CFRSolver:
 
     def _bind_factors(self, n):
         """DCFR: the factor table covers the next n iterations"""
-        if self._factors is not None:
-            self.bufs.desc.dcfr = self._factors.ensure(self.iter_counter + n)
+        self.bufs.desc.dcfr = self.alg.factor_table(self.iter_counter + n)
 
     def _iteration(self, n):
         self._bind_factors(n)
@@ -373,18 +368,16 @@ class CFRSolver:
 
     # ---- checkpoint / resume (the reference's CFR classes keep regrets only inside node objects; WorkerBase.py:23-38 is
     #      a no-op skeleton) - SURVEY.md §8f N1
+    def _identity(self):
+        return {"engine": "levels", **self.alg.identity(), "avg_f64": self.avg_f64, "rank": getattr(self, "rank", 0),
+                "world": getattr(self, "world", 1), "n_nodes": self.ft.n_nodes}
+
     def state_dict(self):
-        return {"engine": "levels", "algo": self.algo_name, "delay": self.delay, "avg_f64": self.avg_f64,
-                "dcfr": list(self.dcfr) if self.dcfr else None, "rank": getattr(self, "rank", 0), "world": getattr(self, "world", 1), "n_nodes": self.ft.n_nodes,
-                "iter_counter": self.iter_counter, "modes": list(self.modes),
+        return {**self._identity(), "iter_counter": self.iter_counter, "modes": list(self.modes),
                 "regret": self.bufs.regret.cpu(), "strat": self.bufs.strat.cpu(), "avg": self.bufs.avg.cpu()}
 
     def load_state_dict(self, state):
-        mine = {"engine": "levels", "algo": self.algo_name, "delay": self.delay, "avg_f64": self.avg_f64,
-                "dcfr": list(self.dcfr) if self.dcfr else None, "rank": getattr(self, "rank", 0), "world": getattr(self, "world", 1), "n_nodes": self.ft.n_nodes}
-        for k, v in mine.items():
-            if state.get(k, v) != v:
-                raise ValueError("checkpoint mismatch on %r: file has %r, this solver %r" % (k, state.get(k), v))
+        algorithm.check_identity(state, self._identity())
         if tuple(state["regret"].shape) != tuple(self.bufs.regret.shape) or state["avg"].dtype != self.bufs.avg.dtype:
             raise ValueError("checkpoint tables do not fit this solver (shape %s vs %s, avg dtype %s vs %s)" % (
                 tuple(state["regret"].shape), tuple(self.bufs.regret.shape), state["avg"].dtype, self.bufs.avg.dtype))
@@ -396,24 +389,22 @@ class CFRSolver:
 
     # ---- evaluation (_CFRBase._log_curr_strat_expl :198-216, _evaluate_avg_strats :218-262)
     def _metric(self, expl):
-        e = [float(expl[p]) * self.ev_normalizer for p in range(2)]
-        return sum(e) / 2
+        return algorithm.seat_averaged(expl, self.ev_normalizer)
 
     def exploitability_current(self):
         if self.persistent:
             return self._metric(self.ops.evaluate(self.modes, do_reach=False))
-        self.ops.value_pass(self.modes, 3, True)
+        self._value_pass_br(self.ops, self.modes)
         return self._metric(self.ops.root_exploitability())
 
     def average_modes(self):
-        if self.algo != nat.ALGO_CFR_PLUS:
-            return [nat.STRAT_AVG_SUM, nat.STRAT_AVG_SUM]
-        if self.iter_counter <= self.delay:
-            raise RuntimeError("CFR+ has no average strategy before iteration delay+1 (CFRPlus.py:33-35)")
-        if self.iter_counter == self.delay + 1:
-            return [nat.STRAT_F32, nat.STRAT_F32]  # avg == copy of the current strategy (CFRPlus.py:83-84)
-        m = nat.STRAT_AVG_F64 if self.avg_f64 else nat.STRAT_AVG_F32
+        m = {algorithm.SUMS: nat.STRAT_AVG_SUM, algorithm.CURRENT: nat.STRAT_F32,
+             algorithm.AVERAGE: nat.STRAT_AVG_F64 if self.avg_f64 else nat.STRAT_AVG_F32}[self.alg.average(self.iter_counter)]
         return [m, m]
+
+    def _value_pass_br(self, ops, modes):
+        """value pass with best responses of both seats over the buffers of `ops` (per-level launches)"""
+        ops.value_pass(modes, 3, True)
 
     def exploitability_average(self):
         if self._eval_bufs is None:
@@ -423,5 +414,5 @@ class CFRSolver:
         if self.persistent:
             return self._metric(self._eval_ops.evaluate(m, do_reach=True))
         self._eval_ops.reach_pass(m)
-        self._eval_ops.value_pass(m, 3, True)
+        self._value_pass_br(self._eval_ops, m)
         return self._metric(self._eval_ops.root_exploitability())

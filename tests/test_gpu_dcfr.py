@@ -114,7 +114,6 @@ def _teacher_forced(spec, stack=20000, grid=0, warm=0, counters=range(4)):
             s.load_natural_tables(ft, orc.regret, orc.avg)
             s.set_trunk_strategy_from_regrets()
             s.iter_counter = t
-            s.g.dcfr = s._factors.ensure(t + 1)
             e1 = e2 = 0.0
             if p == 0:
                 a, b = s.exploitability_current(), orc.exploitability_current()
@@ -171,8 +170,6 @@ def test_board_engine_sums_independent_of_grid_and_shards_equal_one_device():
         parts = [_board_engine(spec, rank=r, world=2, reduce_fn=lambda t: None) for r in range(2)]
         for it in range(3):
             one.iteration(1)
-            for e in parts:
-                e.g.dcfr = e._factors.ensure(e.iter_counter + 1)
             for p in (0, 1):
                 for e in parts:
                     e._update_begin(p)
