@@ -30,8 +30,9 @@ typedef void* prl_stream_t; /* cudaStream_t */
     4: prl_board_sweep / prl_board_trunk take the algorithm; prl_tree_t gained the all-in terminals of two-card games: level_nallin / allin_nodes / allin_pot / allin_tiles /
     allin_partial; 5: prl_board_update_cfrp / prl_board_avg_flush; 6: prl_board_policy_query; 7: second board-engine shape,
     prl_board_layout / prl_board_rows / prl_board_policy_query take the shape; 8: PRL_ALGO_DCFR, prl_buffers_t / prl_board_game_t
-    gained the DCFR factor table `dcfr`) */
-#define PRL_ABI_VERSION 8
+    gained the DCFR factor table `dcfr`; 9: PRL_ALGO_PCFR_PLUS, which reads w_t from that table, prl_board_game_t gained the
+    prediction table `pred`) */
+#define PRL_ABI_VERSION 9
 
 /* node kinds (game/_/tree/_/nodes.py:8-62 + ValueFiller.py:34-62) */
 enum {
@@ -43,11 +44,16 @@ enum {
     PRL_KIND_SHOWDOWN_ALLIN = 5  /* terminal: all-in showdown before the board is complete */
 };
 
-/* algorithms (cfr/VanillaCFR.py, cfr/CFRPlus.py, cfr/LinearCFR.py; Discounted CFR, Brown & Sandholm, AAAI 2019).
+/* algorithms (cfr/VanillaCFR.py, cfr/CFRPlus.py, cfr/LinearCFR.py; Discounted CFR, Brown & Sandholm, AAAI 2019;
+ * Predictive CFR+, Farina, Kroer & Sandholm, AAAI 2021).
  * DCFR, iteration counter i, t = i + 1, factors {a_t, b_t, w_t} = row i of the caller's table `dcfr`: seat p's regret
  * update is x = d + R_old, R_new = x * (x > 0 ? a_t : b_t), the strategy is regret matching of R_new and the average is the
- * reach-weighted sum of strategies with weight w_t (as Linear CFR's with weight t). */
-enum { PRL_ALGO_VANILLA = 0, PRL_ALGO_CFR_PLUS = 1, PRL_ALGO_LINEAR = 2, PRL_ALGO_DCFR = 3 };
+ * reach-weighted sum of strategies with weight w_t (as Linear CFR's with weight t).
+ * PCFR+, same counter: R_new = max(d + R_old, 0) (CFR+'s rule), the strategy is regret matching of the prediction
+ * max(R_new + d, 0) and the average is the reach-weighted sum with weight w_t = column 2 of row i of `dcfr` (columns 0 and 1
+ * are not read).  The level sweeps keep the strategy in `strat`; the board engine keeps the predictions in
+ * prl_board_game_t.pred and reads the strategies of PCFR+ from them. */
+enum { PRL_ALGO_VANILLA = 0, PRL_ALGO_CFR_PLUS = 1, PRL_ALGO_LINEAR = 2, PRL_ALGO_DCFR = 3, PRL_ALGO_PCFR_PLUS = 4 };
 
 /* where a player's strategy comes from in a reach / value pass, and in which precision the reference computes
  * with it (SURVEY.md appendix C) */
@@ -142,7 +148,8 @@ typedef struct {
     void* workspace;          /* DEVICE scratch for the chance-node reductions of two-card games (else NULL) */
     uint64_t workspace_bytes; /* >= 4 * n_chance_per_level * (ceil(max_chance_children / 128) + 1) * ld * 4 bytes */
     const float* dcfr;        /* DEVICE float[n][3] {a_t, b_t, w_t}, row = iteration counter (n > every counter a call
-                                 updates with); read by PRL_ALGO_DCFR only, which fails without it (NULL otherwise) */
+                                 updates with); read by PRL_ALGO_DCFR, and by PRL_ALGO_PCFR_PLUS for w_t only, which fail
+                                 without it (NULL otherwise) */
 } prl_buffers_t;
 
 /* library info */
@@ -265,7 +272,10 @@ typedef struct {
     int64_t* w_total;        /* DEVICE int64[4][n_range]: fixed-point sums over this device's boards of board_mult * root value,
                                 natural hand order.  Update sweep: array 0 = ev of the seat; evaluation sweep of seat p:
                                 arrays 2p = ev, 2p + 1 = ev_br */
-    const float* dcfr;       /* DEVICE float[n][3] {a_t, b_t, w_t} of PRL_ALGO_DCFR as in prl_buffers_t (NULL otherwise) */
+    const float* dcfr;       /* DEVICE float[n][3] {a_t, b_t, w_t} of PRL_ALGO_DCFR as in prl_buffers_t; PRL_ALGO_PCFR_PLUS reads
+                                w_t (column 2) from it (NULL otherwise) */
+    float* pred;             /* DEVICE float[n_rows][ldb] PRL_ALGO_PCFR_PLUS: the predicted regrets max(R + d, 0), laid out as
+                                `regret`; every strategy of a PCFR+ sweep is regret matching of these rows (NULL otherwise) */
 } prl_board_game_t;
 
 /* out[8] = {n_live, ldb, blob bytes per board, byte offset of the int16 hand ids, byte offset of the card rows,
@@ -286,13 +296,15 @@ int prl_board_build_tables(const int32_t* ranks, const uint64_t* board_mask, con
 /* One sweep over all boards for seat p.  eval == 0: update of p's post-deal rows by `algo` (PRL_ALGO_*; iteration iter,
  * CFR+ averaging delay `delay`); eval != 0: values and best-response values of p with the strategies of p / the opponent
  * taken from src_own / src_opp (0 = regret matching of `regret`, 1 = rows of `avg` as they are (CFR+ average), 2 = rows of
- * `avg` normalised (the reach-weighted sums of Vanilla / Linear CFR)).  trunk_reach_opp = DEVICE float[ld]: reach row of the
+ * `avg` normalised (the reach-weighted sums of Vanilla / Linear CFR); PRL_ALGO_PCFR_PLUS: 0 = regret matching of `pred`).  trunk_reach_opp = DEVICE float[ld]: reach row of the
  * opponent at the chance node.  Leaves the fixed-point sums in g->w_total (the arrays it produces are zeroed first).
  * Vanilla / Linear CFR (VanillaCFR.py:54-60, LinearCFR.py:53-59): the average is the sum of strategy x own reach x weight with
  * the reach under the NEW strategy, trunk included - known only after the seat's trunk update.  The contribution of the
  * OPPONENT's last update is therefore added by this sweep (defer_w = its weight, 0 = none pending), which walks those rows
  * anyway; p1_only != 0 does nothing else (flush before the average strategy is evaluated or exported).  DCFR takes the same
- * deferred path, with defer_w = the w_t of the iteration of the opponent's update. */
+ * deferred path, with defer_w = the w_t of the iteration of the opponent's update.  PRL_ALGO_PCFR_PLUS takes it too, with
+ * g->pred: the update reads the own regret and prediction rows and writes R = max(d + R, 0), then Q = max(R + d, 0); every
+ * strategy (opponent, own, flush, evaluation of the current strategy) is regret matching of `pred`.  It fails without pred. */
 int prl_board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, int src_opp, const float* trunk_reach_opp,
                     int iter, int delay, int algo, float defer_w, int p1_only, prl_stream_t stream);
 

@@ -41,7 +41,7 @@ def _stream(dev):
 def supports(game_cls, env_args, algo):
     """True iff the game's abstract tree is one pre-deal trunk + one chance layer + a compiled post-deal shape (Flop5Holdem:
     stacks of 301 chips and more; at 300 and below the preflop raise is all-in and there is no post-deal betting)"""
-    if algo not in algorithm.ALGOS or game_cls.RULES.N_HOLE_CARDS != 2 or game_cls.RULES.N_CARDS_IN_DECK != 52:
+    if algo not in algorithm.ALL or game_cls.RULES.N_HOLE_CARDS != 2 or game_cls.RULES.N_CARDS_IN_DECK != 52:
         return False
     if game_cls.RULES.N_FLOP_CARDS != 5 or os.environ.get("PRL_ENGINE", "board") != "board":
         return False
@@ -271,11 +271,11 @@ class _BoardEngine:
 
 class BoardCFRSolver(_BoardEngine):
     def __init__(self, game_cls, env_args, board_spec=None, algo="CFRPlus", delay=0, device=None, rank=0, world=1,
-                 group=None, grid=0, reduce_fn=None, dcfr=_dcfr.DEFAULT):
+                 group=None, grid=0, reduce_fn=None, dcfr=_dcfr.DEFAULT, pcfr_gamma=algorithm.PCFR_GAMMA):
         self.device = _require_cuda(device)
-        self.alg = algorithm.Algorithm(algo, delay, dcfr, self.device)
+        self.alg = algorithm.Algorithm(algo, delay, dcfr, self.device, pcfr_gamma)
         self.algo_name, self.algo, self.delay, self.dcfr = self.alg.name, self.alg.code, self.alg.delay, self.alg.dcfr
-        self._factors = self.alg.factors  # DCFR's device table (None for the other algorithms), grown by factor_table
+        self._factors = self.alg.factors  # DCFR's / PCFR+'s device table (None for the others), grown by factor_table
         self.rank, self.world, self.group = int(rank), int(world), group
         # cross-rank sum of the fixed-point chance sums, in place; default: torch.distributed all-reduce when world > 1
         self._reduce_fn = reduce_fn
@@ -305,6 +305,10 @@ class BoardCFRSolver(_BoardEngine):
         self.regret = torch.zeros((max(self.n_rows, 1), self.L["ldb"]), dtype=torch.float32, device=dev)
         self.avg = torch.zeros_like(self.regret)
         g.regret, g.avg = self.regret.data_ptr(), self.avg.data_ptr()
+        # PCFR+ only: the predicted regrets max(R + d, 0) of the post-deal rows, laid out as `regret` (every strategy of its
+        # sweeps is regret matching of these rows)
+        self.pred = torch.zeros_like(self.regret) if self.algo == nat.ALGO_PCFR_PLUS else None
+        g.pred = self.pred.data_ptr() if self.pred is not None else None
         # chance sums: two generations of [4][R] int64 (a sweep writes one generation while slow peers may still read the other)
         self._symm = None
         self.collective = "none" if self.world == 1 else "nccl all_reduce(int64)"
@@ -435,7 +439,8 @@ class BoardCFRSolver(_BoardEngine):
         cl = self.chance_level
         if self.algo != nat.ALGO_CFR_PLUS:  # VanillaCFR.py:56-59 / LinearCFR.py:55-58: weight of this update's strategy in the sums
             if not self.fused_trunk:
-                raise RuntimeError("Vanilla / Linear CFR and DCFR on the board engine need the fused trunk (unset PRL_TRUNK=levels)")
+                raise RuntimeError("Vanilla / Linear CFR, DCFR and PCFR+ on the board engine need the fused trunk (unset "
+                                   "PRL_TRUNK=levels)")
             self._pending[p] = self.alg.sum_weight(self.iter_counter)  # THIS iteration's, whichever later sweep adds it
         if self.fused_trunk:
             self._reduce(self.w_total[:1])
@@ -456,6 +461,8 @@ class BoardCFRSolver(_BoardEngine):
             self.iter_counter = 0
             for t in (self.regret, self.avg, self.bufs.regret, self.bufs.strat, self.bufs.avg):
                 t.zero_()
+            if self.pred is not None:
+                self.pred.zero_()
             self._clear_pending()
             self.modes = [nat.STRAT_UNIFORM64, nat.STRAT_UNIFORM64]
             self._reach_trunk(self.bufs, 3, -1, -1, self.modes, self.iter_counter, self.delay)
@@ -508,37 +515,59 @@ class BoardCFRSolver(_BoardEngine):
     # ------------------------------------------------------------------------------------------------ interfaces
     def natural_tables(self, ft):
         """(regret, avg) as natural-order float32 [ft.n_slots, ld] tensors in the slot order of the flat tree `ft` built over
-        THIS rank's boards (for agents, exports and parity tests on small instances)."""
+        THIS rank's boards (for agents, exports and parity tests on small instances); PCFR+: (regret, avg, pred), whose trunk
+        rows are the trunk's stored strategy (regret matching of its predictions, which the trunk does not keep)."""
         assert ft.board_spec.boards.shape[0] == self.n_boards
         self.flush_average()
         nts, out = self.n_trunk_slots, []
+        pairs = [(self.regret, self.bufs.regret), (self.avg, self.bufs.avg)]
+        if self.pred is not None:
+            pairs.append((self.pred, self.bufs.strat))
         with torch.cuda.device(self.device):
-            for tab, trunk_tab in ((self.regret, self.bufs.regret), (self.avg, self.bufs.avg)):
+            for tab, trunk_tab in pairs:
                 nat_tab = torch.zeros((ft.n_slots, self.ld), dtype=torch.float32, device=self.device)
                 self._board_permute(tab, nat_tab, 1, ft)
                 nat_tab[:nts] = trunk_tab[:nts]
                 out.append(nat_tab)
         return out
 
-    def load_natural_tables(self, ft, regret, avg):
-        """inverse of natural_tables (teacher forcing in the parity tests, checkpoints written by the level engine)"""
+    def load_natural_tables(self, ft, regret, avg, pred=None):
+        """inverse of natural_tables (teacher forcing in the parity tests, checkpoints written by the level engine); PCFR+
+        takes the predictions `pred` too: post-deal rows into `self.pred`, and the trunk's stored strategy becomes regret
+        matching of the given trunk rows"""
+        if (pred is None) != (self.pred is None):
+            raise ValueError("load_natural_tables: predictions are given exactly for PCFR+")
         self._clear_pending()  # the given average is complete
         nts, dev = self.n_trunk_slots, self.device
+        triples = [(self.regret, self.bufs.regret, regret), (self.avg, self.bufs.avg, avg)]
+        if pred is not None:
+            triples.append((self.pred, None, pred))
         with torch.cuda.device(dev):
-            for tab, trunk_tab, given in ((self.regret, self.bufs.regret, regret), (self.avg, self.bufs.avg, avg)):
+            for tab, trunk_tab, given in triples:
                 nat_tab = torch.zeros((ft.n_slots, self.ld), dtype=torch.float32, device=dev)
                 nat_tab[:, :given.shape[1]] = torch.as_tensor(given, dtype=torch.float32).to(dev)
                 self._board_permute(tab, nat_tab, 0, ft)
-                trunk_tab[:nts] = nat_tab[:nts]
+                if trunk_tab is not None:
+                    trunk_tab[:nts] = nat_tab[:nts]
+                else:
+                    self._set_trunk_strategy(nat_tab)
 
     def set_trunk_strategy_from_regrets(self):
         """after load_natural_tables: the trunk's stored strategy rows = regret matching of its regret rows, reach rows
-        refreshed (the post-deal rows need nothing: their strategy is never stored)"""
+        refreshed (the post-deal rows need nothing: their strategy is never stored).  PCFR+ sets the trunk's strategy from
+        the predictions load_natural_tables was given instead."""
+        if self.pred is not None:
+            raise RuntimeError("PCFR+: the trunk strategy is regret matching of the predictions given to load_natural_tables")
+        self._set_trunk_strategy(self.bufs.regret)
+
+    def _set_trunk_strategy(self, rows):
+        """the trunk's stored strategy rows = regret matching of the trunk rows of `rows` (natural slot order), reach rows
+        refreshed"""
         ft = self.ft1
         for n in range(self.chance_node + 1):
             if ft.kind[n] <= 1 and ft.first_child[n] >= 0:
                 fs, A = int(ft.first_slot[n]), int(ft.n_children[n])
-                self.bufs.strat[fs:fs + A] = _normalised(self.bufs.regret[fs:fs + A], 0, True)
+                self.bufs.strat[fs:fs + A] = _normalised(rows[fs:fs + A], 0, True)
         self.modes = [nat.STRAT_F32, nat.STRAT_F32]
         with torch.cuda.device(self.device):
             self._reach_trunk(self.bufs, 3, -1, -1, self.modes, self.iter_counter, self.delay)
@@ -551,7 +580,8 @@ class BoardCFRSolver(_BoardEngine):
         self.flush_average()
         return {**self._identity(), "iter_counter": self.iter_counter, "modes": list(self.modes),
                 "regret": self.regret.cpu(), "avg": self.avg.cpu(),
-                "trunk_regret": self.bufs.regret.cpu(), "trunk_strat": self.bufs.strat.cpu(), "trunk_avg": self.bufs.avg.cpu()}
+                "trunk_regret": self.bufs.regret.cpu(), "trunk_strat": self.bufs.strat.cpu(), "trunk_avg": self.bufs.avg.cpu(),
+                **({"pred": self.pred.cpu()} if self.alg.code == nat.ALGO_PCFR_PLUS else {})}
 
     def load_state_dict(self, state):
         algorithm.check_identity(state, self._identity())
@@ -561,6 +591,8 @@ class BoardCFRSolver(_BoardEngine):
         self._clear_pending()  # state_dict() flushes before it exports
         self.regret.copy_(state["regret"])
         self.avg.copy_(state["avg"])
+        if self.alg.code == nat.ALGO_PCFR_PLUS:
+            self.pred.copy_(state["pred"])
         self.bufs.regret.copy_(state["trunk_regret"])
         self.bufs.strat.copy_(state["trunk_strat"])
         self.bufs.avg.copy_(state["trunk_avg"])

@@ -18,10 +18,10 @@ from pokerrl_b200.solver import CFRSolver
 
 
 class CFRBase:
-    _SOLVER_ALGO = None  # "VanillaCFR" | "CFRPlus" | "LinearCFR" | "DCFR"
+    _SOLVER_ALGO = None  # "VanillaCFR" | "CFRPlus" | "LinearCFR" | "DCFR" | "PCFRPlus"
 
     def __init__(self, name, chief_handle, game_cls, agent_bet_set, algo_name, starting_stack_sizes=None,
-                 delay=0, eval_every=1, device=None, avg_f64=False, board_spec=None, dcfr=None):
+                 delay=0, eval_every=1, device=None, avg_f64=False, board_spec=None, dcfr=None, pcfr_gamma=None):
         import os
         avg_f64 = bool(avg_f64) or os.environ.get("PRL_AVG_F64", "0") == "1"  # numpy >= 2 semantics of CFRPlus.py:69-73
         self._name = name
@@ -36,7 +36,8 @@ class CFRBase:
             for s in self._starting_stack_sizes]
         env_cls = get_env_cls_from_str(self._game_cls_str)
         self._env_bldrs = [HistoryEnvBuilder(env_cls=env_cls, env_args=a) for a in self._env_args]
-        self._solvers = [self._make_solver(env_cls, a, delay, device, avg_f64, board_spec, dcfr) for a in self._env_args]
+        self._solvers = [self._make_solver(env_cls, a, delay, device, avg_f64, board_spec, dcfr, pcfr_gamma)
+                         for a in self._env_args]
         self._flat_trees = [getattr(s, "ft", None) for s in self._solvers]  # None: board engine (no node arrays)
         for s, a in zip(self._solvers, self._env_args):
             ft = getattr(s, "ft", None) or s
@@ -53,12 +54,14 @@ class CFRBase:
         self._exp_all_averaged_avg_total = ch.create_experiment(self._name + "_Avg_total_averaged_" + algo_name)
         self._iter_counter = None
 
-    def _make_solver(self, env_cls, env_args, delay, device, avg_f64, board_spec, dcfr=None):
+    def _make_solver(self, env_cls, env_args, delay, device, avg_f64, board_spec, dcfr=None, pcfr_gamma=None):
         """One engine per stack size.  Two-card games launched under torch.distributed (one process per GPU) shard their
         boards over the ranks (pokerrl_b200.distributed); everything else runs on this process's GPU.  dcfr: DCFR's
-        (alpha, beta, gamma), handed to whichever engine runs it."""
+        (alpha, beta, gamma), pcfr_gamma: PCFR+'s gamma, handed to whichever engine runs it."""
         import torch.distributed as dist
         kw = {} if dcfr is None else {"dcfr": dcfr}
+        if pcfr_gamma is not None:
+            kw["pcfr_gamma"] = pcfr_gamma
         multi = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1
         if device is None and multi:  # one process per GPU: this rank's device, not cuda:0
             import os

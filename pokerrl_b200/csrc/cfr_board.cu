@@ -315,9 +315,14 @@ __device__ __forceinline__ void st_stream(float* p, float v) { __stcs(p, v); }
 // left pending.  The strategy of the step of iteration t is regret matching of the regrets the sweep of t wrote, which the
 // seat's next sweep reads and matches for its value backup anyway: there (a.pair) the pending step is applied to the loaded
 // average right before this iteration's, one read and one write of the average rows for two steps.
-template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true>
+// PRED (PCFR+ update form, DEFER family): every strategy is regret matching of the prediction rows G.pred.  P3 loads the own
+// regret rows and the own prediction rows (in the registers the paired form gives its average rows), takes the strategy from
+// the predictions and writes R = max(d + R, 0), then Q = max(R + d, 0).  The average is DEFER's reach-weighted sum (defer_w =
+// w_t).  PCFR+'s evaluation and flush run the EVAL / P1ONLY forms on a copy of the descriptor whose `regret` is `pred`.
+template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true, bool PRED = false>
 __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArgs a) {
     static_assert(!(EVAL && DEFER) && (!P1ONLY || DEFER) && (AVG || (!EVAL && !DEFER)), "variants");
+    static_assert(!PRED || (DEFER && !P1ONLY), "PRED is an update form of the DEFER family");
     using M = SweepSmem<SH>;
     constexpr int NSD = SH::n_sd, NF = SH::n_fold;
     extern __shared__ __align__(128) unsigned char smem[];
@@ -345,7 +350,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
     constexpr size_t kBoardFloats = (size_t)ROWS * kLdb;
     const unsigned char* blob_g = reinterpret_cast<const unsigned char*>(G.tables);
     // tables the two seats' strategies come from (evaluation: regret matching of `regret` or the rows of `avg`)
-    const float* tab_opp = (EVAL && a.src_opp >= 1) ? G.avg : G.regret;
+    const float* tab_opp = PRED ? G.pred : (EVAL && a.src_opp >= 1) ? G.avg : G.regret;
     const float* tab_own = (EVAL && a.src_own >= 1) ? G.avg : G.regret;
     const int asis_opp = (EVAL && a.src_opp == 1) ? 1 : 0, asis_own = (EVAL && a.src_own == 1) ? 1 : 0;
     const bool do_avg = !EVAL && !DEFER && AVG && a.iter >= a.delay;
@@ -394,6 +399,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
     auto prefetch_own = [&](int jj) {
         bulk_prefetch_l2(tab_own + (size_t)jj * kBoardFloats + (size_t)OWN0 * kLdb, NOWN * kLdb * 4);
         if (read_avg) bulk_prefetch_l2(G.avg + (size_t)jj * kBoardFloats + (size_t)OWN0 * kLdb, NOWN * kLdb * 4);
+        if constexpr (PRED) bulk_prefetch_l2(G.pred + (size_t)jj * kBoardFloats + (size_t)OWN0 * kLdb, NOWN * kLdb * 4);
     };
     if (tid == 0 && j < nb) {  // first board's tables
         mbar_expect_tx(&bars[0], kBlobA);
@@ -595,6 +601,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
         const float* own_rows = tab_own + (size_t)j * kBoardFloats + (size_t)OWN0 * kLdb;
         float* reg_rows = G.regret + (size_t)j * kBoardFloats + (size_t)OWN0 * kLdb;
         float* avg_rows = G.avg + (size_t)j * kBoardFloats + (size_t)OWN0 * kLdb;
+        float* pred_rows = PRED ? G.pred + (size_t)j * kBoardFloats + (size_t)OWN0 * kLdb : nullptr;  // PRED: own predictions
         auto p3_pos = [&](int k) -> int { return tid + k * kThreads; };  // strength position of the thread's k-th hand of P3
         float gA[NOWN], aA[NOWN], gB[NOWN], aB[NOWN];
         auto p3_load = [&](int k, float (&g)[NOWN], float (&av)[NOWN]) {
@@ -606,6 +613,10 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
             if (read_avg) {
 #pragma unroll
                 for (int r = 0; r < NOWN; ++r) av[r] = ld_stream(avg_rows + (size_t)r * kLdb + i);
+            }
+            if constexpr (PRED) {  // the own prediction rows ride in the average's registers
+#pragma unroll
+                for (int r = 0; r < NOWN; ++r) av[r] = ld_stream(pred_rows + (size_t)r * kLdb + i);
             }
         };
         p3_load(0, gA, aA);
@@ -730,7 +741,14 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
                         float g[A], s[A];
 #pragma unroll
                         for (int c = 0; c < A; ++c) g[c] = gown[r0 + c];
-                        node_strategy<A>(g, asis_own, s);
+                        if constexpr (PRED) {  // PCFR+: the strategy from the predictions
+                            float q[A];
+#pragma unroll
+                            for (int c = 0; c < A; ++c) q[c] = av[r0 + c];
+                            node_strategy<A>(q, 0, s);
+                        } else {
+                            node_strategy<A>(g, asis_own, s);
+                        }
                         if (pair) {  // s = the pending step's strategy: matching of the same regret rows, same statements
 #pragma unroll
                             for (int c = 0; c < A; ++c) av[r0 + c] = avg_step(a.m_old_due, av[r0 + c], a.m_new_due, s[c]);
@@ -745,6 +763,15 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
                             for (int c = 1; c < A; ++c) b = fmaxf(b, br[fc + c]);
                             br[n] = b;
                         } else {
+                            if constexpr (PRED) {  // PCFR+: R = max(d + R, 0) (CFRPlus.py:37-41), then Q = max(R + d, 0)
+#pragma unroll
+                                for (int c = 0; c < A; ++c) {
+                                    const float d = e[fc + c] - v;
+                                    g[c] = fmaxf(d + g[c], 0.0f);
+                                    st_stream(reg_rows + (size_t)(r0 + c) * kLdb + i, g[c]);
+                                    st_stream(pred_rows + (size_t)(r0 + c) * kLdb + i, fmaxf(g[c] + d, 0.0f));
+                                }
+                            } else {
 #pragma unroll
                             for (int c = 0; c < A; ++c) {
                                 if constexpr (DEFER) {  // VanillaCFR.py:26-27, LinearCFR.py:27-28
@@ -761,6 +788,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
                                 for (int c = 0; c < A; ++c)
                                     st_stream(avg_rows + (size_t)(r0 + c) * kLdb + i, avg_step(a.m_old, av[r0 + c], a.m_new, s[c]));
                             }
+                            }  // !PRED
                         }
                     }
                 }
@@ -1060,7 +1088,9 @@ __device__ __forceinline__ float trunk_sigma(const prl_trunk_t& t, int src, int 
 // peers != NULL: the cross-GPU sum is done HERE - every rank's fixed-point vector sits in symmetric (peer-mapped) memory and
 // is read over NVLink with coalesced 8-byte loads, rank 0 .. n_peers-1 in order (integers: any order gives the same bits),
 // into w_scratch; the caller has placed a cross-rank barrier between the sweep kernels and this launch.
-template <bool EVAL>
+// PRED (PCFR+ update): regrets max(d + R, 0), stored strategy = regret matching of max(R + d, 0), average += s * reach * w_t
+// with w_t = disc[2] (no discount)
+template <bool EVAL, bool PRED = false>
 __global__ void __launch_bounds__(kTrunkThreads) trunk_kernel(const prl_trunk_t t, const long long* __restrict__ w_total,
                                                               const long long* const* __restrict__ peers, int n_peers,
                                                               long long peer_offset, long long* __restrict__ w_scratch,
@@ -1155,6 +1185,22 @@ __global__ void __launch_bounds__(kTrunkThreads) trunk_kernel(const prl_trunk_t 
                     if (EVAL) {
                         b = br_p[(size_t)fc * ld + h];
                         for (int c = 1; c < A; ++c) b = fmaxf(b, br_p[(size_t)(fc + c) * ld + h]);
+                    } else if (PRED) {  // PCFR+: the predictions go through `strat`, then are normalised in place
+                        float ssum = 0.0f;
+                        for (int c = 0; c < A; ++c) {
+                            float* rg = t.regret + (size_t)(fs + c) * ld + h;
+                            const float d = ev_p[(size_t)(fc + c) * ld + h] - v;
+                            const float r = fmaxf(d + *rg, 0.0f);
+                            const float q = fmaxf(r + d, 0.0f);
+                            *rg = r;
+                            t.strat[(size_t)(fs + c) * ld + h] = q;
+                            ssum += q;
+                        }
+                        const float inv = (ssum > 0.0f) ? 1.0f / ssum : 0.0f;
+                        for (int c = 0; c < A; ++c) {
+                            float* st = t.strat + (size_t)(fs + c) * ld + h;
+                            *st = (ssum > 0.0f) ? *st * inv : 1.0f / (float)A;
+                        }
                     } else {  // CFRPlus.py:37-63; VanillaCFR.py:26-52 / LinearCFR.py:27-51: weighted, unclipped, matching on the positive part
                         float ssum = 0.0f;
                         for (int c = 0; c < A; ++c) {
@@ -1193,7 +1239,8 @@ __global__ void __launch_bounds__(kTrunkThreads) trunk_kernel(const prl_trunk_t 
                     if (k == p) {
                         s = t.strat[(size_t)(fs + c) * ld + h];
                         float* a = t.avg + (size_t)(fs + c) * ld + h;
-                        if (algo != PRL_ALGO_CFR_PLUS)  // VanillaCFR.py:56-59, LinearCFR.py:55-58; DCFR: weight w_t
+                        if (PRED) *a = __fadd_rn(*a, __fmul_rn(__fmul_rn(s, r), disc[2]));  // PCFR+: weight w_t
+                        else if (algo != PRL_ALGO_CFR_PLUS)  // VanillaCFR.py:56-59, LinearCFR.py:55-58; DCFR: weight w_t
                             *a = __fadd_rn(*a, __fmul_rn(__fmul_rn(s, r), disc ? disc[2] : rw));
                         else if (iter >= delay) *a = m_old * (*a) + m_new * s;
                     }
@@ -1259,9 +1306,9 @@ int default_grid() {
     return cached[dev];
 }
 
-template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true>
+template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true, bool PRED = false>
 int launch_sweep(const SweepArgs& a, int grid, cudaStream_t s) {
-    auto kern = board_sweep_kernel<SH, P, EVAL, DEFER, P1ONLY, AVG>;
+    auto kern = board_sweep_kernel<SH, P, EVAL, DEFER, P1ONLY, AVG, PRED>;
     constexpr int kSmemBytes = SweepSmem<SH>::kSmemBytes;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);  // per device: set every time
     if (e != cudaSuccess) return prl::check(e, "prl_board_sweep: shared memory opt-in");
@@ -1318,6 +1365,8 @@ extern "C" int prl_board_build_tables(const int32_t* ranks, const uint64_t* boar
 static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, int src_opp, const float* trunk_reach_opp, int iter,
                        int delay, int algo, float defer_w, int p1_only, int due, int now, prl_stream_t stream) {
     if (int e = prl::check_algo(algo, g->dcfr, !eval && !p1_only, "prl_board_sweep")) return e;
+    const bool pred = algo == PRL_ALGO_PCFR_PLUS;
+    if (pred && !g->pred) return prl::fail("prl_board_sweep: PCFR+ needs the prediction table g->pred");
     const bool defer = !eval && algo != PRL_ALGO_CFR_PLUS;
     if (p1_only && !defer) return prl::fail("prl_board_sweep: p1_only is the average flush of Vanilla / Linear CFR");
     const int layout_ok = with_shape(g, [&](auto sh) { return layout_matches<decltype(sh)>(g) ? 1 : 0; });
@@ -1334,6 +1383,9 @@ static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, 
     const int grid = g->grid > 0 ? g->grid : default_grid();
     SweepArgs a;
     a.g = *g;
+    // PCFR+'s strategies are regret matching of the predictions: the evaluation and the flush read them where the other
+    // algorithms read their regrets (their instantiations unchanged); the update form (PRED) reads both tables
+    if (pred && (eval || p1_only)) a.g.regret = g->pred;
     a.trunk_reach_opp = trunk_reach_opp;
     a.iter = iter;
     a.delay = delay;
@@ -1365,6 +1417,8 @@ static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, 
     const int rc = with_shape(g, [&](auto sh) {
         using SH = decltype(sh);
         if (eval) return (p == 0) ? launch_sweep<SH, 0, true>(a, grid, s) : launch_sweep<SH, 1, true>(a, grid, s);
+        if (pred) return (p == 0) ? launch_sweep<SH, 0, false, true, false, true, true>(a, grid, s)
+                                  : launch_sweep<SH, 1, false, true, false, true, true>(a, grid, s);
         if (defer) return (p == 0) ? launch_sweep<SH, 0, false, true>(a, grid, s) : launch_sweep<SH, 1, false, true>(a, grid, s);
         if (step) return (p == 0) ? launch_sweep<SH, 0, false>(a, grid, s) : launch_sweep<SH, 1, false>(a, grid, s);
         return (p == 0) ? launch_sweep<SH, 0, false, false, false, false>(a, grid, s)
@@ -1468,7 +1522,8 @@ extern "C" int prl_board_trunk(const prl_board_game_t* g, const prl_trunk_t* t, 
     if (int e = prl::check_algo(algo, g ? g->dcfr : nullptr, !eval, "prl_board_trunk")) return e;
     if (!g || !t || t->n_nodes < 1 || t->n_nodes > 8) return prl::fail("prl_board_trunk: 1..8 trunk nodes");
     const float rw = prl::regret_weight(algo, iter);
-    const float* disc = prl::dcfr_row(algo, g->dcfr, iter, !eval);
+    const bool pred = algo == PRL_ALGO_PCFR_PLUS && !eval;  // PCFR+ update: w_t from the factor table, no discount
+    const float* disc = pred ? g->dcfr + 3 * (size_t)iter : prl::dcfr_row(algo, g->dcfr, iter, !eval);
     if (with_shape(g, [](auto) { return 0; }) == kNoShape) return prl::fail("prl_board_trunk: the post-deal subtree has no compiled shape");
     if (t->n_range != kRange || g->n_deck != kDeck) return prl::fail("prl_board_trunk: 52-card deck / 1326 hands only");
     if (eval && !out_expl) return prl::fail("prl_board_trunk: out_expl missing");
@@ -1485,6 +1540,10 @@ extern "C" int prl_board_trunk(const prl_board_game_t* g, const prl_trunk_t* t, 
     if (eval)
         trunk_kernel<true><<<1, kTrunkThreads, 0, (cudaStream_t)stream>>>(*t, w, pp, n_peers, (long long)peer_offset, ws, sym_perm, n_sym,
                                                                        inv_scale, -1, iter, delay, m_old, m_new, algo, rw, disc, out_expl);
+    else if (pred)
+        trunk_kernel<false, true><<<1, kTrunkThreads, 0, (cudaStream_t)stream>>>(*t, w, pp, n_peers, (long long)peer_offset, ws, sym_perm,
+                                                                              n_sym, inv_scale, p, iter, delay, m_old, m_new, algo, rw, disc,
+                                                                              out_expl);
     else
         trunk_kernel<false><<<1, kTrunkThreads, 0, (cudaStream_t)stream>>>(*t, w, pp, n_peers, (long long)peer_offset, ws, sym_perm, n_sym,
                                                                         inv_scale, p, iter, delay, m_old, m_new, algo, rw, disc, out_expl);

@@ -164,8 +164,9 @@ __device__ __forceinline__ int card_rank(int h, int b, int pair_bonus) {
 }
 
 // ------------------------------------------------------------------------------------------------ reach (top-down)
-// Lane = (parent node of level d, hand); writes element h of the reach rows of the children (level d+1).
-template <int R, bool UPDATE_AVG>
+// Lane = (parent node of level d, hand); writes element h of the reach rows of the children (level d+1).  PRED: PCFR+
+// (c.algo == PRL_ALGO_PCFR_PLUS), whose average is DCFR's reach-weighted sum with weight w_t.
+template <int R, bool UPDATE_AVG, bool PRED = false>
 __device__ __forceinline__ void reach_group(const Ctx& c, const int lo, const int hi, const int grp) {
     const LaneMap<R> L;
     const int t = lo + grp * LaneMap<R>::NPW + L.g;
@@ -210,7 +211,7 @@ __device__ __forceinline__ void reach_group(const Ctx& c, const int lo, const in
                 const bool avg_f64 = upd && c.algo == PRL_ALGO_CFR_PLUS && c.avg_f64 && c.iter >= c.delay;
                 float* avf = (float*)c.B.avg + (size_t)fs * ld + h;
                 double* avd = (double*)c.B.avg + (size_t)fs * ld + h;
-                const float w = (upd && c.algo == PRL_ALGO_DCFR) ? c.B.dcfr[3 * (size_t)c.iter + 2] : (float)(c.iter + 1);
+                const float w = (upd && (PRED || c.algo == PRL_ALGO_DCFR)) ? c.B.dcfr[3 * (size_t)c.iter + 2] : (float)(c.iter + 1);
                 for (int k0 = 0; k0 < A; k0 += kChunk) {  // loads of a chunk first, then the stores
                     float s[kChunk], av[kChunk];
                     double ad[kChunk];
@@ -232,7 +233,7 @@ __device__ __forceinline__ void reach_group(const Ctx& c, const int lo, const in
                             } else if (avg_f32) {
                                 float a;
                                 if (c.algo == PRL_ALGO_CFR_PLUS) a = (float)m_old * av[j] + (float)m_new * s[j];
-                                else if (c.algo == PRL_ALGO_LINEAR || c.algo == PRL_ALGO_DCFR) a = av[j] + x * w;  // LinearCFR.py:56-61
+                                else if (PRED || c.algo == PRL_ALGO_LINEAR || c.algo == PRL_ALGO_DCFR) a = av[j] + x * w;  // LinearCFR.py:56-61
                                 else a = av[j] + x;                                      // VanillaCFR.py:57-62
                                 avf[(size_t)(k0 + j) * ld] = a;
                             }
@@ -312,8 +313,8 @@ __device__ __forceinline__ float fold_children(const float* __restrict__ col, in
 
 // Seat p acts at this node and is being updated, A children (compile time): node value with the current strategy,
 // regret update (_CFRBase.py:146-185) and regret matching (CFRPlus.py:43-63 and siblings).  Everything the lane needs
-// is requested before the first use; returns the node value.
-template <int A>
+// is requested before the first use; returns the node value.  PRED: PCFR+'s regret and matching of its prediction.
+template <int A, bool PRED>
 __device__ __forceinline__ float update_own(const Ctx& c, int md, const float* __restrict__ ecol, int fs, int h) {
     const int ld = c.T.ld;
     float* rcol = c.B.regret + (size_t)fs * ld + h;
@@ -338,8 +339,26 @@ __device__ __forceinline__ float update_own(const Ctx& c, int md, const float* _
         for (int k = 1; k < A; ++k) acc = acc + strat_f64(c, md, fs, k, A, h) * (double)e[k];
         v = (float)acc;
     }
-    const prl::RegretW w = prl::regret_w(c);
     float ssum = 0.0f;
+    if constexpr (PRED) {
+        float pr[A];  // the predictions max(R_new + d, 0)
+#pragma unroll
+        for (int k = 0; k < A; ++k) {
+            const float d = e[k] - v;
+            rg[k] = prl::pcfr_regret(d, rg[k]);
+            pr[k] = prl::pcfr_prediction(rg[k], d);
+            ssum = (k == 0) ? pr[k] : ssum + pr[k];
+        }
+        const float uni = (float)(1.0 / (double)A);
+        const float den = (ssum > 0.0f) ? ssum : 1.0f;
+#pragma unroll
+        for (int k = 0; k < A; ++k) {
+            rcol[k * ld] = rg[k];
+            scol[k * ld] = (ssum > 0.0f) ? pr[k] / den : uni;
+        }
+        return v;
+    }
+    const prl::RegretW w = prl::regret_w(c);
 #pragma unroll
     for (int k = 0; k < A; ++k) {
         rg[k] = prl::regret_step(c.algo, e[k] - v, rg[k], w);
@@ -358,8 +377,8 @@ __device__ __forceinline__ float update_own(const Ctx& c, int md, const float* _
 }
 
 // ------------------------------------------------------------------------------------------------ value (bottom-up)
-// Lane = (node of level d, hand); reads element h of its children's rows (level d+1).
-template <int R, int NS, bool WITH_BR, bool UPDATE>
+// Lane = (node of level d, hand); reads element h of its children's rows (level d+1).  PRED: the update is PCFR+'s.
+template <int R, int NS, bool WITH_BR, bool UPDATE, bool PRED = false>
 __device__ __forceinline__ void value_group(const Ctx& c, const int lo, const int hi, const int grp) {
     constexpr int kRegA = 8;  // children of an updated node kept in registers (wider nodes stream)
     const LaneMap<R> L;
@@ -394,14 +413,14 @@ __device__ __forceinline__ void value_group(const Ctx& c, const int lo, const in
             if (upd && A <= kRegA) {
                 // warps are uniform in A (work list sorted by kind, n_children): jump to the exactly-unrolled variant
                 switch (A) {
-                    case 1: v = update_own<1>(c, md, ecol, fs, h); break;
-                    case 2: v = update_own<2>(c, md, ecol, fs, h); break;
-                    case 3: v = update_own<3>(c, md, ecol, fs, h); break;
-                    case 4: v = update_own<4>(c, md, ecol, fs, h); break;
-                    case 5: v = update_own<5>(c, md, ecol, fs, h); break;
-                    case 6: v = update_own<6>(c, md, ecol, fs, h); break;
-                    case 7: v = update_own<7>(c, md, ecol, fs, h); break;
-                    default: v = update_own<8>(c, md, ecol, fs, h); break;
+                    case 1: v = update_own<1, PRED>(c, md, ecol, fs, h); break;
+                    case 2: v = update_own<2, PRED>(c, md, ecol, fs, h); break;
+                    case 3: v = update_own<3, PRED>(c, md, ecol, fs, h); break;
+                    case 4: v = update_own<4, PRED>(c, md, ecol, fs, h); break;
+                    case 5: v = update_own<5, PRED>(c, md, ecol, fs, h); break;
+                    case 6: v = update_own<6, PRED>(c, md, ecol, fs, h); break;
+                    case 7: v = update_own<7, PRED>(c, md, ecol, fs, h); break;
+                    default: v = update_own<8, PRED>(c, md, ecol, fs, h); break;
                 }
             } else {
                 if (mode_is_f32(md)) {
@@ -434,16 +453,29 @@ __device__ __forceinline__ void value_group(const Ctx& c, const int lo, const in
                     const prl::RegretW w = prl::regret_w(c);
                     float ssum = 0.0f;
                     for (int k = 0; k < A; ++k) {
-                        const float rp = fmaxf(prl::regret_step(c.algo, ecol[(size_t)k * ld] - v, rcol[(size_t)k * ld], w), 0.0f);
+                        float rp;
+                        if constexpr (PRED) {
+                            const float d = ecol[(size_t)k * ld] - v;
+                            rp = prl::pcfr_prediction(prl::pcfr_regret(d, rcol[(size_t)k * ld]), d);
+                        } else {
+                            rp = fmaxf(prl::regret_step(c.algo, ecol[(size_t)k * ld] - v, rcol[(size_t)k * ld], w), 0.0f);
+                        }
                         ssum = (k == 0) ? rp : ssum + rp;
                     }
                     const float uni = (float)(1.0 / (double)A);
                     const float den = (ssum > 0.0f) ? ssum : 1.0f;
                     for (int k = 0; k < A; ++k) {
-                        const float r = prl::regret_step(c.algo, ecol[(size_t)k * ld] - v, rcol[(size_t)k * ld], w);
-                        rcol[(size_t)k * ld] = r;
-                        const float q = fmaxf(r, 0.0f) / den;
-                        scol[(size_t)k * ld] = (ssum > 0.0f) ? q : uni;
+                        if constexpr (PRED) {
+                            const float d = ecol[(size_t)k * ld] - v;
+                            const float r = prl::pcfr_regret(d, rcol[(size_t)k * ld]);
+                            rcol[(size_t)k * ld] = r;
+                            scol[(size_t)k * ld] = (ssum > 0.0f) ? prl::pcfr_prediction(r, d) / den : uni;
+                        } else {
+                            const float r = prl::regret_step(c.algo, ecol[(size_t)k * ld] - v, rcol[(size_t)k * ld], w);
+                            rcol[(size_t)k * ld] = r;
+                            const float q = fmaxf(r, 0.0f) / den;
+                            scol[(size_t)k * ld] = (ssum > 0.0f) ? q : uni;
+                        }
                     }
                 }
             }
@@ -454,16 +486,16 @@ __device__ __forceinline__ void value_group(const Ctx& c, const int lo, const in
 }
 
 // ---- one launch per level (any tree size): one warp per group of NPW nodes --------------------------------------------
-template <int R, bool UPDATE_AVG>
+template <int R, bool UPDATE_AVG, bool PRED = false>
 __global__ void __launch_bounds__(kThreads) reach_level_kernel(const Ctx c) {
     const int grp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (grp < groups_of(c.hi - c.lo, LaneMap<R>::NPW)) reach_group<R, UPDATE_AVG>(c, c.lo, c.hi, grp);
+    if (grp < groups_of(c.hi - c.lo, LaneMap<R>::NPW)) reach_group<R, UPDATE_AVG, PRED>(c, c.lo, c.hi, grp);
 }
 
-template <int R, int NS, bool WITH_BR, bool UPDATE>
+template <int R, int NS, bool WITH_BR, bool UPDATE, bool PRED = false>
 __global__ void __launch_bounds__(kThreads) value_level_kernel(const Ctx c) {
     const int grp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (grp < groups_of(c.hi - c.lo, LaneMap<R>::NPW)) value_group<R, NS, WITH_BR, UPDATE>(c, c.lo, c.hi, grp);
+    if (grp < groups_of(c.hi - c.lo, LaneMap<R>::NPW)) value_group<R, NS, WITH_BR, UPDATE, PRED>(c, c.lo, c.hi, grp);
 }
 
 // ---- persistent cooperative kernels: whole sweeps / iterations in ONE launch, grid barrier between levels ------------
@@ -498,8 +530,8 @@ __device__ __forceinline__ void root_exploitability(const prl_tree_t& T, const p
 }
 
 // THREADS: block size = threads per SM (one block per SM): 512 at 128 registers per thread.  A 1024-thread / 64-register
-// instantiation was no faster on the B_5 tree and was removed.
-template <int R, int NS, int THREADS>
+// instantiation was no faster on the B_5 tree and was removed.  PRED: PCFR+ (c.algo == PRL_ALGO_PCFR_PLUS).
+template <int R, int NS, int THREADS, bool PRED = false>
 __global__ void __launch_bounds__(THREADS, 1) cfr_iterations_kernel(Ctx c, const Levels lv, const int n_iters) {
     cg::grid_group grid = cg::this_grid();
     // warp w of block b takes 32-entry chunk (w * gridDim + b) of the kind-sorted work list: consecutive chunks go to
@@ -516,14 +548,14 @@ __global__ void __launch_bounds__(THREADS, 1) cfr_iterations_kernel(Ctx c, const
             c.upd_p = p;
             for (int d = lv.n_levels - 1; d >= 0; --d) {
                 const int lo = lv.start[d], hi = lv.start[d + 1], ng = groups_of(hi - lo, NPW);
-                for (int grp = gwarp; grp < ng; grp += nwarps) value_group<R, NS, false, true>(c, lo, hi, grp);
+                for (int grp = gwarp; grp < ng; grp += nwarps) value_group<R, NS, false, true, PRED>(c, lo, hi, grp);
                 grid.sync();
                 stamp(lv, ts);
             }
             c.mode[p] = PRL_STRAT_F32;
             for (int d = 0; d < last; ++d) {
                 const int lo = lv.start[d], hi = lo + lv.nonterm[d], ng = groups_of(hi - lo, NPW);
-                for (int grp = gwarp; grp < ng; grp += nwarps) reach_group<R, true>(c, lo, hi, grp);
+                for (int grp = gwarp; grp < ng; grp += nwarps) reach_group<R, true, PRED>(c, lo, hi, grp);
                 grid.sync();
                 stamp(lv, ts);
             }
@@ -587,13 +619,15 @@ int check_tree(const prl_tree_t* t) {
 
 template <int R>
 void launch_reach(const Ctx& c, int nodes, bool update_avg, cudaStream_t s) {
-    if (update_avg) PRL_LAUNCH((reach_level_kernel<R, true>), nodes, LaneMap<R>::NPW, s, c);
+    if (update_avg && c.algo == PRL_ALGO_PCFR_PLUS) PRL_LAUNCH((reach_level_kernel<R, true, true>), nodes, LaneMap<R>::NPW, s, c);
+    else if (update_avg) PRL_LAUNCH((reach_level_kernel<R, true>), nodes, LaneMap<R>::NPW, s, c);
     else PRL_LAUNCH((reach_level_kernel<R, false>), nodes, LaneMap<R>::NPW, s, c);
 }
 
 template <int R>
 void launch_value(const Ctx& c, int nodes, bool with_br, bool update, cudaStream_t s) {
-    if (update) PRL_LAUNCH((value_level_kernel<R, 2, false, true>), nodes, LaneMap<R>::NPW, s, c);
+    if (update && c.algo == PRL_ALGO_PCFR_PLUS) PRL_LAUNCH((value_level_kernel<R, 2, false, true, true>), nodes, LaneMap<R>::NPW, s, c);
+    else if (update) PRL_LAUNCH((value_level_kernel<R, 2, false, true>), nodes, LaneMap<R>::NPW, s, c);
     else if (with_br) PRL_LAUNCH((value_level_kernel<R, 2, true, false>), nodes, LaneMap<R>::NPW, s, c);
     else PRL_LAUNCH((value_level_kernel<R, 2, false, false>), nodes, LaneMap<R>::NPW, s, c);
 }
@@ -708,13 +742,14 @@ int coop_grid(K kernel, int* grid, int threads = kPThreads) {
     return 0;
 }
 
-template <int R>
+template <int R, bool PRED>
 int launch_iterations(Ctx& c, Levels& lv, int n_iters, cudaStream_t s) {
     int grid = 0;
     void* args[] = {&c, &lv, &n_iters};
-    if (int e = coop_grid(cfr_iterations_kernel<R, 2, kPThreads>, &grid)) return e;
+    if (int e = coop_grid(cfr_iterations_kernel<R, 2, kPThreads, PRED>, &grid)) return e;
     prl::count_launch();
-    return prl::check(cudaLaunchCooperativeKernel((void*)cfr_iterations_kernel<R, 2, kPThreads>, dim3(grid), dim3(kPThreads), args, 0, s),
+    return prl::check(cudaLaunchCooperativeKernel((void*)cfr_iterations_kernel<R, 2, kPThreads, PRED>, dim3(grid), dim3(kPThreads), args, 0,
+                                                  s),
                       "prl_cfr_iterations");
 }
 
@@ -752,8 +787,10 @@ extern "C" int prl_cfr_iterations(const prl_tree_t* tree, const prl_buffers_t* b
     Ctx c{*tree, *buf, 0, 0, 0, {strat_mode[0], strat_mode[1]}, algo, 0, iter0, delay, avg_f64};
     Levels lv;
     if (int e = make_levels(tree, &lv)) return e;
-    return tree->n_range == 6 ? launch_iterations<6>(c, lv, n_iters, (cudaStream_t)stream)
-                              : launch_iterations<24>(c, lv, n_iters, (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (algo == PRL_ALGO_PCFR_PLUS)
+        return tree->n_range == 6 ? launch_iterations<6, true>(c, lv, n_iters, s) : launch_iterations<24, true>(c, lv, n_iters, s);
+    return tree->n_range == 6 ? launch_iterations<6, false>(c, lv, n_iters, s) : launch_iterations<24, false>(c, lv, n_iters, s);
 }
 
 extern "C" int prl_evaluate(const prl_tree_t* tree, const prl_buffers_t* buf, const int* strat_mode, int do_reach,

@@ -105,9 +105,11 @@ struct RegretMatch {
     }
 };
 
-// average-strategy update of table row ap from the row's strategy s and the child's reach r
+// average-strategy update of table row ap from the row's strategy s and the child's reach r.  PRED: PCFR+, whose average is
+// DCFR's reach-weighted sum with weight w_t.
+template <bool PRED>
 __device__ __forceinline__ void avg_update(const Ctx2& c, float* ap, const F4& s, const F4& r) {
-    if (c.algo == PRL_ALGO_CFR_PLUS) {  // CFRPlus.py:65-87 (float table)
+    if (!PRED && c.algo == PRL_ALGO_CFR_PLUS) {  // CFRPlus.py:65-87 (float table)
         if (c.iter >= c.delay) {
             F4 a = ld4(ap);
 #pragma unroll
@@ -117,7 +119,7 @@ __device__ __forceinline__ void avg_update(const Ctx2& c, float* ap, const F4& s
     } else {
         F4 a = ld4(ap);
         const float w = (c.algo == PRL_ALGO_LINEAR) ? (float)(c.iter + 1)                  // LinearCFR.py:56-61
-                        : (c.algo == PRL_ALGO_DCFR) ? c.B.dcfr[3 * (size_t)c.iter + 2] : 1.0f;
+                        : (PRED || c.algo == PRL_ALGO_DCFR) ? c.B.dcfr[3 * (size_t)c.iter + 2] : 1.0f;
 #pragma unroll
         for (int i = 0; i < 4; ++i) a.v[i] = a.v[i] + r.v[i] * w;  // VanillaCFR.py:57-62
         st4(ap, a);
@@ -127,7 +129,7 @@ __device__ __forceinline__ void avg_update(const Ctx2& c, float* ap, const F4& s
 // ------------------------------------------------------------------------------------------------ reach (top-down)
 // reach rows of node n for hands h0..h0+3 (StrategyFiller.py:118-146 generalised).  Structure of n: parent par, n's table
 // row `slot`, first table row fs of its siblings, kind pk and fan-out A of the parent (read only when par >= 0).
-template <bool UPDATE_AVG>
+template <bool UPDATE_AVG, bool PRED = false>
 __device__ __forceinline__ void reach_rows(const Ctx2& c, int n, int h0, int par, int slot, int fs, int pk, int A) {
     const int ld = c.T.ld, R = c.T.n_range;
     const size_t N = (size_t)c.T.n_nodes;
@@ -153,7 +155,7 @@ __device__ __forceinline__ void reach_rows(const Ctx2& c, int n, int h0, int par
                 const F4 s = strat4(c, c.mode[q], slot, fs, A, h0);
 #pragma unroll
                 for (int i = 0; i < 4; ++i) r.v[i] = s.v[i] * rp.v[i];
-                if (UPDATE_AVG && q == c.upd_p) avg_update(c, (float*)c.B.avg + (size_t)slot * ld + h0, s, r);
+                if (UPDATE_AVG && q == c.upd_p) avg_update<PRED>(c, (float*)c.B.avg + (size_t)slot * ld + h0, s, r);
             } else {
                 r = rp;
             }
@@ -163,7 +165,7 @@ __device__ __forceinline__ void reach_rows(const Ctx2& c, int n, int h0, int par
 }
 
 // block x = child node n of the level, thread = four hands; structure through the parent -> first_child -> slot chain
-template <bool UPDATE_AVG>
+template <bool UPDATE_AVG, bool PRED = false>
 __global__ void __launch_bounds__(kVecThreads) reach2_kernel(const Ctx2 c) {
     const int n = c.lo + blockIdx.x;
     const int h0 = 4 * (blockIdx.y * blockDim.x + threadIdx.x);
@@ -175,7 +177,7 @@ __global__ void __launch_bounds__(kVecThreads) reach2_kernel(const Ctx2 c) {
         pk = c.T.kind[par];
         A = c.T.n_children[par];
     }
-    reach_rows<UPDATE_AVG>(c, n, h0, par, c.T.slot[n], fs, pk, A);
+    reach_rows<UPDATE_AVG, PRED>(c, n, h0, par, c.T.slot[n], fs, pk, A);
 }
 
 // ---- v2 row kernels: one CTA per node (ceil(R / 4) threads rounded up to a warp), node structure from ONE 16-byte
@@ -183,19 +185,20 @@ __global__ void __launch_bounds__(kVecThreads) reach2_kernel(const Ctx2 c) {
 constexpr int kRowThreadsMax = 352;  // 1326 hands / 4 per thread = 332 -> 11 warps
 
 // node_rec2[n] = {parent, slot of n, first slot of the parent's children, kind(parent) | n_children(parent) << 8}
-template <bool UPDATE_AVG>
+template <bool UPDATE_AVG, bool PRED = false>
 __global__ void __launch_bounds__(kRowThreadsMax, 4) reach2_kernel_v2(const Ctx2 c) {
     const int n = c.lo + blockIdx.x;
     const int h0 = 4 * threadIdx.x;
     if (h0 >= c.T.n_range) return;
     const int4 rec = reinterpret_cast<const int4*>(c.T.node_rec2)[n];
-    reach_rows<UPDATE_AVG>(c, n, h0, rec.x, rec.y, rec.z, rec.w & 0xff, rec.w >> 8);
+    reach_rows<UPDATE_AVG, PRED>(c, n, h0, rec.x, rec.y, rec.z, rec.w & 0xff, rec.w >> 8);
 }
 
 // ------------------------------------------------------------------------------------------------ decision nodes (bottom-up)
 // regrets + regret matching of the seat's own node with the A child rows held in registers (each row is loaded once);
-// same operations in the same order as the loops of value_rows -> identical results
-template <int A>
+// same operations in the same order as the loops of value_rows -> identical results.  PRED: PCFR+'s regret, and regret
+// matching of its prediction max(R_new + d, 0)
+template <int A, bool PRED>
 __device__ __forceinline__ F4 own_node_update(const Ctx2& c, int fs, int h0, const float* ecol) {
     const size_t ld = c.T.ld;
     float* rcol = c.B.regret + (size_t)fs * ld + h0;
@@ -212,8 +215,27 @@ __device__ __forceinline__ F4 own_node_update(const Ctx2& c, int fs, int h0, con
 #pragma unroll
         for (int i = 0; i < 4; ++i) v.v[i] += s.v[i] * e[k].v[i];
     }
-    const prl::RegretW w = prl::regret_w(c);
     F4 ssum = splat(0.0f);
+    if constexpr (PRED) {  // each row's regrets are stored as soon as they are known; rg[k] then holds the prediction
+#pragma unroll
+        for (int k = 0; k < A; ++k) {
+            F4 pr;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const float d = e[k].v[i] - v.v[i];
+                rg[k].v[i] = prl::pcfr_regret(d, rg[k].v[i]);
+                pr.v[i] = prl::pcfr_prediction(rg[k].v[i], d);
+                ssum.v[i] += pr.v[i];
+            }
+            st4(rcol + (size_t)k * ld, rg[k]);
+            rg[k] = pr;
+        }
+        const RegretMatch rm(ssum, A);
+#pragma unroll
+        for (int k = 0; k < A; ++k) st4(scol + (size_t)k * ld, rm(rg[k]));
+        return v;
+    }
+    const prl::RegretW w = prl::regret_w(c);
 #pragma unroll
     for (int k = 0; k < A; ++k) {
 #pragma unroll
@@ -233,8 +255,8 @@ __device__ __forceinline__ F4 own_node_update(const Ctx2& c, int fs, int h0, con
 
 // ValueFiller.py:80-93 + _CFRBase.py:146-185 + regret matching of decision node n for hands h0..h0+3, given its
 // structure: first child fc, first table row fs of the children, kind, fan-out A.  REG_ROWS: the updating seat's own
-// node with fan-out 2..4 takes the register-resident own_node_update
-template <bool WITH_BR, bool UPDATE, bool REG_ROWS>
+// node with fan-out 2..4 takes the register-resident own_node_update.  PRED: the update is PCFR+'s.
+template <bool WITH_BR, bool UPDATE, bool REG_ROWS, bool PRED = false>
 __device__ __forceinline__ void value_rows(const Ctx2& c, int n, int fc, int fs, int kind, int A, int h0) {
     const int ld = c.T.ld;
     const size_t N = (size_t)c.T.n_nodes;
@@ -258,9 +280,9 @@ __device__ __forceinline__ void value_rows(const Ctx2& c, int n, int fc, int fs,
                     for (int i = 0; i < 4; ++i) vbr.v[i] += e.v[i];
                 }
         } else if (REG_ROWS && UPDATE && p == c.upd_p && A >= 2 && A <= 4 && c.mode[p] == PRL_STRAT_F32) {
-            if (A == 2) v = own_node_update<2>(c, fs, h0, ecol);
-            else if (A == 3) v = own_node_update<3>(c, fs, h0, ecol);
-            else v = own_node_update<4>(c, fs, h0, ecol);
+            if (A == 2) v = own_node_update<2, PRED>(c, fs, h0, ecol);
+            else if (A == 3) v = own_node_update<3, PRED>(c, fs, h0, ecol);
+            else v = own_node_update<4, PRED>(c, fs, h0, ecol);
         } else {
             const int m = c.mode[p];
             for (int k = 0; k < A; ++k) {
@@ -285,16 +307,35 @@ __device__ __forceinline__ void value_rows(const Ctx2& c, int n, int fc, int fs,
                 for (int k = 0; k < A; ++k) {  // pass A: positive regret mass (new regrets are recomputed in pass B)
                     const F4 e = ld4(ecol + (size_t)k * ld), rg = ld4(rcol + (size_t)k * ld);
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) ssum.v[i] += fmaxf(prl::regret_step(c.algo, e.v[i] - v.v[i], rg.v[i], w), 0.0f);
+                    for (int i = 0; i < 4; ++i) {
+                        if constexpr (PRED) {
+                            const float d = e.v[i] - v.v[i];
+                            ssum.v[i] += prl::pcfr_prediction(prl::pcfr_regret(d, rg.v[i]), d);
+                        } else {
+                            ssum.v[i] += fmaxf(prl::regret_step(c.algo, e.v[i] - v.v[i], rg.v[i], w), 0.0f);
+                        }
+                    }
                 }
                 const RegretMatch rm(ssum, A);
                 for (int k = 0; k < A; ++k) {  // pass B: store regrets and the regret-matching strategy
                     const F4 e = ld4(ecol + (size_t)k * ld);
                     F4 rg = ld4(rcol + (size_t)k * ld);
+                    if constexpr (PRED) {
+                        F4 pr;
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) rg.v[i] = prl::regret_step(c.algo, e.v[i] - v.v[i], rg.v[i], w);
-                    st4(rcol + (size_t)k * ld, rg);
-                    st4(scol + (size_t)k * ld, rm(rg));
+                        for (int i = 0; i < 4; ++i) {
+                            const float d = e.v[i] - v.v[i];
+                            rg.v[i] = prl::pcfr_regret(d, rg.v[i]);
+                            pr.v[i] = prl::pcfr_prediction(rg.v[i], d);
+                        }
+                        st4(rcol + (size_t)k * ld, rg);
+                        st4(scol + (size_t)k * ld, rm(pr));
+                    } else {
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) rg.v[i] = prl::regret_step(c.algo, e.v[i] - v.v[i], rg.v[i], w);
+                        st4(rcol + (size_t)k * ld, rg);
+                        st4(scol + (size_t)k * ld, rm(rg));
+                    }
                 }
             }
         }
@@ -304,22 +345,22 @@ __device__ __forceinline__ void value_rows(const Ctx2& c, int n, int fc, int fs,
 }
 
 // block x = work-list entry t -> decision node n, thread = four hands; structure through order / first_child / slot
-template <bool WITH_BR, bool UPDATE>
+template <bool WITH_BR, bool UPDATE, bool PRED = false>
 __global__ void __launch_bounds__(kVecThreads) value2_kernel(const Ctx2 c) {
     const int h0 = 4 * (blockIdx.y * blockDim.x + threadIdx.x);
     if (h0 >= c.T.n_range) return;
     const int n = c.T.order[c.lo + blockIdx.x];
     const int kind = c.T.kind[n], fc = c.T.first_child[n], A = c.T.n_children[n];
-    value_rows<WITH_BR, UPDATE, false>(c, n, fc, c.T.slot[fc], kind, A, h0);
+    value_rows<WITH_BR, UPDATE, false, PRED>(c, n, fc, c.T.slot[fc], kind, A, h0);
 }
 
 // work_rec2[t] = {node, first child, first slot of the children, kind | n_children << 8} of work-list entry t
-template <bool WITH_BR, bool UPDATE>
+template <bool WITH_BR, bool UPDATE, bool PRED = false>
 __global__ void __launch_bounds__(kRowThreadsMax, 3) value2_kernel_v2(const Ctx2 c) {
     const int h0 = 4 * threadIdx.x;
     if (h0 >= c.T.n_range) return;
     const int4 rec = reinterpret_cast<const int4*>(c.T.work_rec2)[c.lo + blockIdx.x];
-    value_rows<WITH_BR, UPDATE, true>(c, rec.x, rec.y, rec.z, rec.w & 0xff, rec.w >> 8, h0);
+    value_rows<WITH_BR, UPDATE, true, PRED>(c, rec.x, rec.y, rec.z, rec.w & 0xff, rec.w >> 8, h0);
 }
 
 // ------------------------------------------------------------------------------------------------ chance nodes (bottom-up)
@@ -920,12 +961,15 @@ inline int row_threads(const prl_tree_t& T) {
 void launch_reach_level(const Ctx2& c, bool update_avg, cudaStream_t s) {
     const prl_tree_t& T = c.T;
     const int rt = row_threads(T);
+    const bool pred = update_avg && c.algo == PRL_ALGO_PCFR_PLUS;
     if (T.node_rec2 && rt) {
-        if (update_avg) reach2_kernel_v2<true><<<c.n, rt, 0, s>>>(c);
+        if (pred) reach2_kernel_v2<true, true><<<c.n, rt, 0, s>>>(c);
+        else if (update_avg) reach2_kernel_v2<true><<<c.n, rt, 0, s>>>(c);
         else reach2_kernel_v2<false><<<c.n, rt, 0, s>>>(c);
     } else {
         const dim3 g((unsigned)c.n, (unsigned)((T.n_range + 4 * kVecThreads - 1) / (4 * kVecThreads)));
-        if (update_avg) reach2_kernel<true><<<g, kVecThreads, 0, s>>>(c);
+        if (pred) reach2_kernel<true, true><<<g, kVecThreads, 0, s>>>(c);
+        else if (update_avg) reach2_kernel<true><<<g, kVecThreads, 0, s>>>(c);
         else reach2_kernel<false><<<g, kVecThreads, 0, s>>>(c);
     }
     prl::count_launch();
@@ -1034,13 +1078,16 @@ int value_levels2(Ctx2 c, bool with_br, bool update, int d_hi, int d_lo, int cha
             c.lo = lo;
             c.n = n_dec;
             const int rt = row_threads(T);
+            const bool pred = update && c.algo == PRL_ALGO_PCFR_PLUS;
             if (T.work_rec2 && rt) {
-                if (update) value2_kernel_v2<false, true><<<n_dec, rt, 0, s>>>(c);
+                if (pred) value2_kernel_v2<false, true, true><<<n_dec, rt, 0, s>>>(c);
+                else if (update) value2_kernel_v2<false, true><<<n_dec, rt, 0, s>>>(c);
                 else if (with_br) value2_kernel_v2<true, false><<<n_dec, rt, 0, s>>>(c);
                 else value2_kernel_v2<false, false><<<n_dec, rt, 0, s>>>(c);
             } else {
                 const dim3 g((unsigned)n_dec, (unsigned)((T.n_range + 4 * kVecThreads - 1) / (4 * kVecThreads)));
-                if (update) value2_kernel<false, true><<<g, kVecThreads, 0, s>>>(c);
+                if (pred) value2_kernel<false, true, true><<<g, kVecThreads, 0, s>>>(c);
+                else if (update) value2_kernel<false, true><<<g, kVecThreads, 0, s>>>(c);
                 else if (with_br) value2_kernel<true, false><<<g, kVecThreads, 0, s>>>(c);
                 else value2_kernel<false, false><<<g, kVecThreads, 0, s>>>(c);
             }

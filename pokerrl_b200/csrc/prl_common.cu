@@ -25,8 +25,10 @@ void count_launch() { ++g_launches; }
 
 int check_algo(int algo, const float* dcfr, bool updates, const char* where) {
     char msg[256];
-    if (algo < PRL_ALGO_VANILLA || algo > PRL_ALGO_DCFR) snprintf(msg, sizeof(msg), "%s: bad algo %d", where, algo);
+    if (algo < PRL_ALGO_VANILLA || algo > PRL_ALGO_PCFR_PLUS) snprintf(msg, sizeof(msg), "%s: bad algo %d", where, algo);
     else if (updates && algo == PRL_ALGO_DCFR && !dcfr) snprintf(msg, sizeof(msg), "%s: DCFR needs the factor table dcfr", where);
+    else if (updates && algo == PRL_ALGO_PCFR_PLUS && !dcfr)
+        snprintf(msg, sizeof(msg), "%s: PCFR+ needs the weight table dcfr (w_t in column 2)", where);
     else return 0;
     return fail(msg);
 }

@@ -13,7 +13,8 @@ int check(cudaError_t e, const char* where);
 // counts kernel launches issued by this library (prl_launch_count())
 void count_launch();
 
-// 0 if `algo` is a PRL_ALGO_* code and, where the call updates, DCFR has its factor table; otherwise fails naming `where`
+// 0 if `algo` is a PRL_ALGO_* code and, where the call updates, DCFR / PCFR+ have the factor table; otherwise fails naming
+// `where`
 int check_algo(int algo, const float* dcfr, bool updates, const char* where);
 // CFR+'s averaging weights of iteration iter (CFRPlus.py:68-73): (0, 1) at iter == delay, whose step copies the strategy
 // (and below delay, which has no step)
@@ -55,4 +56,9 @@ __device__ __forceinline__ float regret_step(int algo, float d, float old, const
     }
     return d + old;                                              // VanillaCFR.py:26-30
 }
+
+// PCFR+ (the level sweeps' PRED instantiations): the regret is CFR+'s, r_new = max(d + R_old, 0), and regret matching reads
+// the prediction max(r_new + d, 0) - the last instantaneous regret added to the new regret - instead of r_new
+__device__ __forceinline__ float pcfr_regret(float d, float old) { return fmaxf(d + old, 0.0f); }
+__device__ __forceinline__ float pcfr_prediction(float r_new, float d) { return fmaxf(r_new + d, 0.0f); }
 }  // namespace prl

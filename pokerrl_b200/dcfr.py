@@ -8,6 +8,9 @@ Iteration counter i (0-based, the engines' iter_counter), t = i + 1:
 each computed in float64 and rounded once to float32.  The kernels read them from a device table float32[n][3] indexed by
 the counter (prl_buffers_t.dcfr / prl_board_game_t.dcfr), so a persistent launch over many iterations needs no host step.
 DCFR(1, 1, 1) gives R_D(t) = R_L(t) / (t + 1) and the average sums of Linear CFR.
+
+Predictive CFR+ weighs its average sums with the same w_t = t^gamma: its device table is the factor table of
+pcfr_params(gamma), of which the kernels read column 2 only.
 """
 import math
 
@@ -28,6 +31,23 @@ def check_params(alpha, beta, gamma):
     return p
 
 
+def check_gamma(gamma):
+    """PCFR+'s gamma as a float; ValueError unless it is a finite number"""
+    try:
+        g = float(gamma)
+    except (TypeError, ValueError):
+        raise ValueError("PCFR+ gamma must be a number, got %r" % (gamma,)) from None
+    if not math.isfinite(g):
+        raise ValueError("PCFR+ gamma must be finite, got %r" % (g,))
+    return g
+
+
+def pcfr_params(gamma):
+    """the (alpha, beta, gamma) of PCFR+'s factor table: w_t = t^gamma in column 2 as DCFR's; alpha = beta = 1 fill the
+    unread columns 0 and 1"""
+    return (1.0, 1.0, check_gamma(gamma))
+
+
 def factors(alpha, beta, gamma, n):
     """float32 [n, 3]: row i = {a_t, b_t, w_t} of iteration counter i (t = i + 1).  ValueError if a w_t is not finite in
     float32."""
@@ -41,7 +61,7 @@ def factors(alpha, beta, gamma, n):
         out = np.stack([disc(alpha), disc(beta), t ** gamma], axis=1).astype(np.float32)
     bad = ~np.isfinite(out[:, 2])
     if bad.any():
-        raise ValueError("DCFR gamma = %r: the average weight t^gamma of iteration t = %d is not finite in float32"
+        raise ValueError("gamma = %r: the average weight t^gamma of iteration t = %d is not finite in float32"
                          % (gamma, int(np.argmax(bad)) + 1))
     return out
 

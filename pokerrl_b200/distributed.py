@@ -15,6 +15,7 @@ import torch
 import torch.distributed as dist
 
 from pokerrl_b200 import _native as nat
+from pokerrl_b200 import algorithm
 from pokerrl_b200 import dcfr as _dcfr
 from pokerrl_b200.game.flat_tree import FlatTree
 from pokerrl_b200.game.holdem_boards import BoardSpec
@@ -52,7 +53,8 @@ class ShardedCFRSolver(CFRSolver):
     world == 1 (or no process group) runs the same split schedule without communication."""
 
     def __init__(self, game_cls, env_args, board_spec, algo="CFRPlus", delay=0, device=None, rank=0, world=1,
-                 group=None, root_actions=None, dcfr=_dcfr.DEFAULT):
+                 group=None, root_actions=None, dcfr=_dcfr.DEFAULT,
+                 pcfr_gamma=algorithm.PCFR_GAMMA):
         self.rank, self.world, self.group = rank, world, group
         ft = FlatTree(game_cls, env_args, board_spec=shard_board_spec(board_spec, rank, world) if world > 1 else board_spec,
                       root_actions=root_actions)
@@ -60,7 +62,8 @@ class ShardedCFRSolver(CFRSolver):
         if world > 1 and (ft.kind == nat.KIND_SHOWDOWN_ALLIN).any():
             raise NotImplementedError("all-in showdowns before the board is complete run out over ALL boards below them: "
                                       "not available with the boards sharded over ranks (run this tree on one GPU)")
-        super().__init__(ft, algo=algo, delay=delay, device=device, avg_f64=False, persistent=False, dcfr=dcfr)
+        super().__init__(ft, algo=algo, delay=delay, device=device, avg_f64=False, persistent=False, dcfr=dcfr,
+                         pcfr_gamma=pcfr_gamma)
         # levels holding BOUNDARY chance nodes: chance nodes right below the replicated trunk (no deal above them), whose
         # children - the boards of the first chance layer - are spread over the ranks.  Deeper chance nodes are local.
         self._n_chance, self._n_boundary = {}, {}

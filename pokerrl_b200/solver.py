@@ -320,12 +320,13 @@ class CFRSolver:
     strategy is a separate, optional evaluation (the reference does both every iteration).
     """
 
-    def __init__(self, ft, algo="CFRPlus", delay=0, device=None, avg_f64=False, persistent=True, dcfr=_dcfr.DEFAULT):
+    def __init__(self, ft, algo="CFRPlus", delay=0, device=None, avg_f64=False, persistent=True, dcfr=_dcfr.DEFAULT,
+                 pcfr_gamma=algorithm.PCFR_GAMMA):
         self.persistent = bool(persistent)  # one cooperative launch per call instead of one launch per tree level
         self.ft = ft
-        self.alg = algorithm.Algorithm(algo, delay, dcfr, _require_cuda(device))
+        self.alg = algorithm.Algorithm(algo, delay, dcfr, _require_cuda(device), pcfr_gamma)
         self.algo_name, self.algo, self.delay, self.dcfr = self.alg.name, self.alg.code, self.alg.delay, self.alg.dcfr
-        self._factors = self.alg.factors  # DCFR's device table (None for the other algorithms), grown by factor_table
+        self._factors = self.alg.factors  # DCFR's / PCFR+'s device table (None for the others), grown by factor_table
         self.avg_f64 = bool(avg_f64) and self.algo == nat.ALGO_CFR_PLUS
         self.dtree = DeviceTree(ft, device)
         self.bufs = TreeBuffers(self.dtree, avg_dtype=torch.float64 if self.avg_f64 else torch.float32)
@@ -346,7 +347,7 @@ class CFRSolver:
             self._iteration(n)
 
     def _bind_factors(self, n):
-        """DCFR: the factor table covers the next n iterations"""
+        """DCFR / PCFR+: the factor table covers the next n iterations"""
         self.bufs.desc.dcfr = self.alg.factor_table(self.iter_counter + n)
 
     def _iteration(self, n):

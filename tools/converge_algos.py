@@ -1,6 +1,8 @@
-"""Exploitability against solve time of CFR+ (delay 0), Linear CFR and Discounted CFR on full Flop5Holdem (board engine).
+"""Exploitability against solve time of CFR+ (delay 0), Linear CFR, Discounted CFR and Predictive CFR+ on full Flop5Holdem
+(board engine).
 
-    python tools/converge_algos.py --budget 150 --eval-every 20 [--marks 15,30,60,120,150] [--dcfr 1.5,0,2] [--boards N]
+    python tools/converge_algos.py --budget 150 --eval-every 20 [--marks 15,30,60,120,150] [--dcfr 1.5,0,2] [--pcfr-gamma 2]
+                                  [--algos CFRPlus,LinearCFR,DCFR,PCFRPlus] [--boards N]
 
 Each algorithm runs alone on the GPU for the same solve-time budget (seconds of CFR iterations, evaluation excluded); every
 --eval-every iterations the exact exploitability of its average strategy (mbb/g, the number the project reports) is
@@ -31,13 +33,13 @@ def device_info():
     return info
 
 
-def run(algo, spec, budget, eval_every, dcfr):
+def run(algo, spec, budget, eval_every, dcfr, pcfr_gamma):
     import torch
     from pokerrl_b200.board_engine import BoardCFRSolver
     from pokerrl_b200.game import games
     g = games.Flop5Holdem
     args = g.ARGS_CLS(n_seats=2, starting_stack_sizes_list=[20000, 20000], bet_sizes_list_as_frac_of_pot=[1.0])
-    s = BoardCFRSolver(g, args, spec, algo=algo, dcfr=dcfr)
+    s = BoardCFRSolver(g, args, spec, algo=algo, dcfr=dcfr, pcfr_gamma=pcfr_gamma)
     s.iteration(2)  # warm-up of every kernel, then a fresh start
     s.reset()
     torch.cuda.synchronize()
@@ -60,6 +62,8 @@ def main():
     ap.add_argument("--eval-every", type=int, default=20)
     ap.add_argument("--marks", default="15,30,60,120,150", help="solve-time marks (s) of the reported exploitability")
     ap.add_argument("--dcfr", default="1.5,0,2", help="DCFR alpha,beta,gamma")
+    ap.add_argument("--pcfr-gamma", type=float, default=2.0, help="PCFR+ gamma (average weight t^gamma)")
+    ap.add_argument("--algos", default="CFRPlus,LinearCFR,DCFR,PCFRPlus", help="which algorithms, in this order")
     ap.add_argument("--boards", type=int, default=0, help="debugging: the first N board classes only")
     a = ap.parse_args()
     import torch
@@ -75,8 +79,11 @@ def main():
     marks = [float(x) for x in a.marks.split(",")]
     out = dict(device_info(), workload="Flop5Holdem full game (%d board classes), stack 20000, pot-size bets" % len(spec.boards),
                budget_solve_s=a.budget, eval_every=a.eval_every, algorithms={})
-    for label, algo in (("CFR+ delay 0", "CFRPlus"), ("Linear CFR", "LinearCFR"), ("DCFR%r" % (dcfr,), "DCFR")):
-        r = run(algo, spec, a.budget, a.eval_every, dcfr)
+    labels = {"CFRPlus": "CFR+ delay 0", "LinearCFR": "Linear CFR", "DCFR": "DCFR%r" % (dcfr,),
+              "PCFRPlus": "PCFR+(gamma %g)" % a.pcfr_gamma}
+    for algo in a.algos.split(","):
+        label = labels[algo]
+        r = run(algo, spec, a.budget, a.eval_every, dcfr, a.pcfr_gamma)
         at = {}
         for m in marks:
             done = [c for c in r["curve"] if c["solve_s"] <= m]
