@@ -31,8 +31,9 @@ typedef void* prl_stream_t; /* cudaStream_t */
     allin_partial; 5: prl_board_update_cfrp / prl_board_avg_flush; 6: prl_board_policy_query; 7: second board-engine shape,
     prl_board_layout / prl_board_rows / prl_board_policy_query take the shape; 8: PRL_ALGO_DCFR, prl_buffers_t / prl_board_game_t
     gained the DCFR factor table `dcfr`; 9: PRL_ALGO_PCFR_PLUS, which reads w_t from that table, prl_board_game_t gained the
-    prediction table `pred`) */
-#define PRL_ABI_VERSION 9
+    prediction table `pred`; 10: restricted Nash response, prl_board_game_t gained the model reach table `rnr_reach` and the
+    mixing probability `rnr_p`, prl_trunk_t the model's trunk reach `reach_model` and `rnr_p`) */
+#define PRL_ABI_VERSION 10
 
 /* node kinds (game/_/tree/_/nodes.py:8-62 + ValueFiller.py:34-62) */
 enum {
@@ -276,6 +277,10 @@ typedef struct {
                                 w_t (column 2) from it (NULL otherwise) */
     float* pred;             /* DEVICE float[n_rows][ldb] PRL_ALGO_PCFR_PLUS: the predicted regrets max(R + d, 0), laid out as
                                 `regret`; every strategy of a PCFR+ sweep is regret matching of these rows (NULL otherwise) */
+    float* rnr_reach;        /* DEVICE float[n_boards][n_sd][ldb] restricted Nash response (CFR+ only): reach of the fixed model
+                                (the opponent of the sweep's seat) at the board's n_sd showdown terminals, strength order, deal
+                                probability and the model's trunk reach included; NULL: a plain sweep.  See prl_board_sweep. */
+    float rnr_p;             /* probability of the model in the opponent's mixture, [0, 1] */
 } prl_board_game_t;
 
 /* out[8] = {n_live, ldb, blob bytes per board, byte offset of the int16 hand ids, byte offset of the card rows,
@@ -304,7 +309,12 @@ int prl_board_build_tables(const int32_t* ranks, const uint64_t* board_mask, con
  * anyway; p1_only != 0 does nothing else (flush before the average strategy is evaluated or exported).  DCFR takes the same
  * deferred path, with defer_w = the w_t of the iteration of the opponent's update.  PRL_ALGO_PCFR_PLUS takes it too, with
  * g->pred: the update reads the own regret and prediction rows and writes R = max(d + R, 0), then Q = max(R + d, 0); every
- * strategy (opponent, own, flush, evaluation of the current strategy) is regret matching of `pred`.  It fails without pred. */
+ * strategy (opponent, own, flush, evaluation of the current strategy) is regret matching of `pred`.  It fails without pred.
+ * Restricted Nash response (g->rnr_reach != NULL, PRL_ALGO_CFR_PLUS only; Johanson, Zinkevich & Bowling, NIPS 2007): the
+ * opponent's reach at the showdown terminals is the sweep's own (from trunk_reach_opp, which the caller scales by 1 - rnr_p)
+ * plus rnr_p * rnr_reach, at the fold terminals the same combination through the fold identity.  The update (here or through
+ * prl_board_update_cfrp) and the evaluation read rnr_reach; p1_only != 0 instead WRITES rnr_reach: the opponent's reach at the
+ * showdown terminals under the rows of `avg` as they are (the model) and trunk_reach_opp (the model's), nothing else. */
 int prl_board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, int src_opp, const float* trunk_reach_opp,
                     int iter, int delay, int algo, float defer_w, int p1_only, prl_stream_t stream);
 
@@ -343,6 +353,11 @@ typedef struct {
     float* regret;  /* DEVICE float[n_slots][ld] trunk tables (natural hand order) */
     float* strat;
     float* avg;
+    const float* reach_model; /* restricted Nash response, DEVICE float[2][n_buf_nodes][ld] laid out as `reach`: the fixed model's
+                                 trunk reach.  Update form: the opponent's reach at the fold terminals is
+                                 (1 - rnr_p) * reach + rnr_p * reach_model.  Evaluation form: out_expl = DEVICE float[6], entries 2 + p
+                                 and 4 + p the root value and best-response value of seat p (reach-weighted sums).  NULL: plain. */
+    float rnr_p;
 } prl_trunk_t;
 
 /* peers != NULL fuses the ONE collective of the path into this launch: peers = DEVICE array of n_peers pointers to every rank's

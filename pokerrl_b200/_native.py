@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("PRL_LIB_PATH") or os.path.join(_HERE, "lib", "libpoke
 # enums of include/pokerrl_b200.h
 KIND_P0, KIND_P1, KIND_CHANCE, KIND_FOLD, KIND_SHOWDOWN, KIND_SHOWDOWN_ALLIN = range(6)
 ALGO_VANILLA, ALGO_CFR_PLUS, ALGO_LINEAR, ALGO_DCFR, ALGO_PCFR_PLUS = 0, 1, 2, 3, 4
-ABI_VERSION = 9  # include/pokerrl_b200.h: PRL_ABI_VERSION
+ABI_VERSION = 10  # include/pokerrl_b200.h: PRL_ABI_VERSION
 STRAT_F32, STRAT_UNIFORM64, STRAT_AVG_F64, STRAT_AVG_SUM, STRAT_AVG_F32 = range(5)
 
 
@@ -50,7 +50,8 @@ class PrlBoardGame(C.Structure):
                 ("n_children", C.c_int8 * 16), ("acted_last", C.c_int8 * 16), ("pot", C.c_float * 16),
                 ("row0", C.c_int64 * 16), ("row_m", C.c_int32 * 16),
                 ("tables", C.c_void_p), ("board_prob", C.c_void_p), ("board_mult", C.c_void_p), ("regret", C.c_void_p),
-                ("avg", C.c_void_p), ("w_private", C.c_void_p), ("w_total", C.c_void_p), ("dcfr", C.c_void_p), ("pred", C.c_void_p)]
+                ("avg", C.c_void_p), ("w_private", C.c_void_p), ("w_total", C.c_void_p), ("dcfr", C.c_void_p), ("pred", C.c_void_p),
+                ("rnr_reach", C.c_void_p), ("rnr_p", C.c_float)]
 
 
 class PrlTrunk(C.Structure):
@@ -58,7 +59,8 @@ class PrlTrunk(C.Structure):
                 ("n_range", C.c_int32), ("mode", C.c_int32 * 2), ("eq_const", C.c_float),
                 ("kind", C.c_int8 * 8), ("first_child", C.c_int8 * 8), ("n_children", C.c_int8 * 8), ("acted_last", C.c_int8 * 8),
                 ("first_slot", C.c_int32 * 8), ("pot", C.c_float * 8), ("hand_cards", C.c_void_p), ("reach", C.c_void_p),
-                ("ev", C.c_void_p), ("ev_br", C.c_void_p), ("regret", C.c_void_p), ("strat", C.c_void_p), ("avg", C.c_void_p)]
+                ("ev", C.c_void_p), ("ev_br", C.c_void_p), ("regret", C.c_void_p), ("strat", C.c_void_p), ("avg", C.c_void_p),
+                ("reach_model", C.c_void_p), ("rnr_p", C.c_float)]
 
 
 class PrlEnvCfg(C.Structure):

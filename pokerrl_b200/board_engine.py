@@ -156,6 +156,27 @@ def _normalised(x, dim, matching):
     return torch.where(ok, x / torch.where(ok, tot, torch.ones_like(tot)), torch.full_like(x, 1.0 / x.shape[dim]))
 
 
+def _sum_to_one(x, dim):
+    """x divided by its sums along `dim` in float64, rounded to x's dtype; uniform where the sum is not positive (the
+    fold identity of the restricted Nash response's sweep needs rows that sum to one)"""
+    d = x.double()
+    tot = d.sum(dim=dim, keepdim=True)
+    ok = tot > 0
+    return torch.where(ok, d / torch.where(ok, tot, torch.ones_like(tot)), torch.full_like(d, 1.0 / d.shape[dim])).to(x.dtype)
+
+
+def _decision_row_groups(st, local_rows):
+    """for every post-deal decision node, the row indices (on one board) of its children"""
+    return [[local_rows[c][0] for c in range(st["first_child"][d], st["first_child"][d] + st["n_children"][d])]
+            for d in _decision_locals(st)]
+
+
+def _trunk_decisions(ft, chance_node):
+    """(first slot, actions) of every trunk decision node of the flat tree `ft`"""
+    return [(int(ft.first_slot[n]), int(ft.n_children[n])) for n in range(chance_node + 1)
+            if ft.kind[n] <= 1 and ft.first_child[n] >= 0]
+
+
 class _BoardEngine:
     """What the solver and the policy evaluator share: the pre-deal trunk, swept by prl_board_trunk / the level kernels over
     its own small buffers, the descriptor `g` of the post-deal subtrees of the boards, and the one call site of each board
@@ -600,6 +621,159 @@ class BoardCFRSolver(_BoardEngine):
             self._reach_trunk(self.bufs, 3, -1, -1, self.modes, self.iter_counter, self.delay)
 
 
+def rnr_probability(p):
+    """the model's probability of a restricted Nash response as float32, ValueError unless it is finite and in [0, 1]"""
+    p = float(p)
+    if not (math.isfinite(p) and 0.0 <= p <= 1.0):
+        raise ValueError("the model's probability p must be a finite number in [0, 1], got %r" % p)
+    return float(np.float32(p))
+
+
+def rnr_identity(seat, p, model_digest):
+    """the checkpoint keys a restricted Nash response game adds to CFR+'s"""
+    return {"rnr_seat": int(seat), "rnr_p": float(p), "rnr_model": model_digest}
+
+
+def device_digest(tensors):
+    """an integer digest of the bits of float32 device tensors, computed on the device in chunks"""
+    acc, mask = 0, (1 << 61) - 1
+    for k, t in enumerate(tensors):
+        flat = t.reshape(-1).view(torch.int32)
+        for a in range(0, flat.numel(), 1 << 24):
+            v = flat[a:a + (1 << 24)].to(torch.int64)
+            w = torch.arange(a + 1, a + 1 + v.numel(), dtype=torch.int64, device=t.device) * 2654435761 + k
+            acc = (acc * 1000003 + int((v * w).sum())) & mask
+    return acc
+
+
+class BoardRNRSolver(BoardCFRSolver):
+    """One game of a restricted Nash response (Johanson, Zinkevich & Bowling, "Computing Robust Counter-Strategies", NIPS
+    2007) on the board engine: seat `seat` (the exploiter) plays against an opponent that is, with probability p drawn before
+    the deal and seen only by the opponent, a fixed model, and otherwise a free strategy.  Both learn by CFR+ (delay as
+    CFRPlus).  The exploiter's values are linear in the opponent's reach, so its update is CFR+'s against the mixed reach
+    (1 - p) * free + p * model:
+      * the model's reach at every board's showdown terminals, trunk reach and deal included, is computed once
+        (`model_reach`, float32 [n_boards * n_sd, 1088], BoardPolicyEvaluator.model_reach) and never changes; the sweep adds
+        p times it to the free copy's, whose trunk reach row the host scales by 1 - p (prl_board_sweep, rnr_reach);
+      * the trunk mixes the opponent's reach at its fold terminals with the model's trunk reach (`trunk_model`).
+    The free copy's update is CFR+'s unchanged: its counterfactual values are 1 - p times those it computes, which scales its
+    regrets by a constant and leaves regret matching as it is.  At p = 1 it is skipped; at p = 0 the exploiter runs the plain
+    CFR+ sweep and trunk.  The model's tables are filled by the owner (RestrictedNashResponse) before the first iteration."""
+
+    def __init__(self, game_cls, env_args, seat, p, board_spec=None, delay=0, device=None, grid=0, share_boards=None):
+        """share_boards: another BoardRNRSolver over the same board spec and device whose per-board tables (blobs, deal
+        probabilities, multiplicities; read-only after set-up) this one uses instead of building its own"""
+        if seat not in (0, 1):
+            raise ValueError("the exploiter's seat is 0 or 1")
+        self.seat, self.p = int(seat), rnr_probability(p)
+        if self.p > 0.0 and os.environ.get("PRL_TRUNK", "fused") == "levels":
+            # the level-kernel trunk has no mixed form: the exploiter's trunk regrets would ignore the model
+            raise ValueError("the restricted Nash response needs the fused trunk (unset PRL_TRUNK=levels)")
+        self._q = float(np.float32(1.0) - np.float32(self.p))  # 1 - p as the trunk kernel computes it
+        self._rnr_trunk = False
+        self._share = share_boards
+        super().__init__(game_cls, env_args, board_spec, algo="CFRPlus", delay=delay, device=device, grid=grid)
+        dev = self.device
+        self.n_sd = sum(1 for k in self.st["kind"][:self.st["n_local"]] if k == nat.KIND_SHOWDOWN)
+        self.model_reach = torch.zeros((max(self.n_boards * self.n_sd, 1), self.L["ldb"]), dtype=torch.float32, device=dev)
+        self.trunk_model = torch.zeros_like(self.bufs.reach)
+        self.model_digest = None
+        self._opp_row = torch.zeros(self.ld, dtype=torch.float32, device=dev)  # the free copy's trunk reach row times 1 - p
+        self._expl = torch.zeros(6, dtype=torch.float32, device=dev)  # prl_trunk_t.reach_model: the evaluation's root values
+
+    def _setup_boards(self, capacity):
+        if self._share is None:
+            return super()._setup_boards(capacity)
+        sh = self._share
+        if sh.n_boards != capacity or not np.array_equal(sh.boards, self.boards) or sh.device != self.device:
+            raise ValueError("share_boards: another board spec or device")
+        self.t_blob, self.t_prob, self.t_mult = sh.t_blob, sh.t_prob, sh.t_mult
+        self.g.tables, self.g.board_prob, self.g.board_mult = sh.g.tables, sh.g.board_prob, sh.g.board_mult
+
+    def _load_boards(self, boards, prob, mult):
+        if self._share is None:
+            return super()._load_boards(boards, prob, mult)
+        self.g.n_boards = boards.shape[0]  # the shared tables are built
+
+    def set_model(self, trunk_model):
+        """after model_reach is filled: the model's trunk reach rows, and the digest that names the model in checkpoints"""
+        self.trunk_model.copy_(trunk_model)
+        with torch.cuda.device(self.device):
+            self.model_digest = device_digest([self.model_reach, self.trunk_model])
+
+    def _rnr_game(self, p):
+        g = nat.PrlBoardGame.from_buffer_copy(self.g)
+        g.rnr_reach, g.rnr_p = self.model_reach.data_ptr(), p
+        return g
+
+    def _skipped(self, p):
+        return p != self.seat and self.p == 1.0  # the free copy never plays
+
+    def _board_update_cfrp(self, p, due, now):
+        if p != self.seat or self.p == 0.0:
+            return super()._board_update_cfrp(p, due, now)
+        free = self.bufs.reach.view(2, -1, self.ld)[1 - p, self.chance_node]
+        torch.mul(free, self._q, out=self._opp_row)
+        nat.call("prl_board_update_cfrp", C.byref(self._rnr_game(self.p)), p, C.c_void_p(self._opp_row.data_ptr()),
+                 self.iter_counter, self.delay, due, now, _stream(self.device))
+
+    def _trunk(self, bufs, modes, evaluate, p):
+        self._rnr_trunk = not evaluate and p == self.seat and self.p > 0.0
+        try:
+            super()._trunk(bufs, modes, evaluate, p)
+        finally:
+            self._rnr_trunk = False
+
+    def _trunk_desc(self, bufs, modes):
+        t = super()._trunk_desc(bufs, modes)
+        if self._rnr_trunk:
+            t.reach_model, t.rnr_p = self.trunk_model.data_ptr(), self.p
+        return t
+
+    def _update_begin(self, p):
+        if not self._skipped(p):
+            super()._update_begin(p)
+
+    def _update_end(self, p):
+        if not self._skipped(p):
+            super()._update_end(p)
+
+    def rnr_values(self):
+        """(exploitation, exploitability) of the exploiter's average strategy in chips: its value against the model, and the
+        value of a best response of the other seat to it (prl_board_sweep with rnr_reach at rnr_p = 1 for the first, the
+        plain evaluation sweep of the other seat for the second, one prl_board_trunk evaluation with reach_model for both)"""
+        if self.model_digest is None:
+            raise RuntimeError("the model's tables are not set")
+        if self.iter_counter == 0:
+            raise RuntimeError("no average strategy before the first iteration")
+        m, src = {algorithm.CURRENT: (nat.STRAT_F32, SRC_REGRET),
+                  algorithm.AVERAGE: (nat.STRAT_AVG_F32, SRC_AVG)}[self.alg.average(self.iter_counter)]
+        s, o = self.seat, 1 - self.seat
+        with torch.cuda.device(self.device):
+            if self._eval_bufs is None:
+                self._eval_bufs = TreeBuffers(self.trunk, share=self.bufs)
+            self.flush_average()
+            bufs = self._eval_bufs
+            self._reach_trunk(bufs, 3, -1, -1, [m, m], self.iter_counter, self.delay)
+            bufs.reach[o].copy_(self.trunk_model[o])  # the exploiter's opponent is the model
+            self._opp_row.zero_()  # the model's reach is all in model_reach
+            nat.call("prl_board_sweep", C.byref(self._rnr_game(1.0)), s, 1, src, src, C.c_void_p(self._opp_row.data_ptr()),
+                     self.iter_counter, self.delay, nat.ALGO_CFR_PLUS, 0.0, 0, _stream(self.device))
+            self._board_sweep(bufs, o, True, src, src, self.iter_counter, self.delay, nat.ALGO_CFR_PLUS)
+            self._reduce(self.w_total)
+            self._rnr_trunk = True
+            try:
+                self._board_trunk(bufs, [m, m], True, -1, self.iter_counter, self.delay, nat.ALGO_CFR_PLUS)
+            finally:
+                self._rnr_trunk = False
+            self._next_generation()
+            e = self._expl.cpu().numpy().astype(np.float64)
+        return float(e[2 + s]), float(e[4 + o])
+
+    def _identity(self):
+        return {**super()._identity(), **rnr_identity(self.seat, self.p, self.model_digest)}
+
+
 # ==================================================================================================================== policy evaluation
 def board_keys(boards):
     """int64 key of each board: its sorted cards packed base 64 (holdem_boards.canonical_boards)"""
@@ -683,11 +857,59 @@ class BoardPolicyEvaluator(_BoardEngine):
         pt.build_structure()
         return pt
 
+    def _chunks(self, agent, tick, normalise=False):
+        """the agent's strategy over the spec, chunk by chunk: for the boards lo .. hi of each chunk (yielded with the time
+        tick() last returned), their tables bound to `g` and the agent's post-deal rows in self.rows, strength order; from the
+        first chunk on, the trunk's rows in bufs.avg and the reach of both seats in bufs.reach.  normalise: every decision
+        node's rows divided by their sum in float64, then rounded to float32 (a model that the fold identity of the sweep
+        holds for), where the sum is positive"""
+        import time
+        R, s, nts = self.R, self.spec, self.n_trunk_slots
+        for lo in range(0, self.n_boards_total, self.chunk):
+            hi = min(lo + self.chunk, self.n_boards_total)
+            t0 = time.perf_counter()
+            pt = self._chunk_tree(lo, hi)
+            ft = pt.flat
+            tab = self.nat_tab[:ft.n_slots]
+            got = pt.agent_strategy_table(agent, out=tab)
+            if not isinstance(got, torch.Tensor):  # answered node by node on the host
+                tab[:, :R].copy_(torch.from_numpy(np.ascontiguousarray(got, np.float32)))
+            t0 = tick("agent query", t0)
+            self._load_boards(s.boards[lo:hi], s.board_prob[lo:hi], s.board_mult[lo:hi])
+            self._board_permute(self.rows, tab, 0, ft)
+            if normalise:
+                rows = self.rows[:(hi - lo) * self.rows_per_board].view(hi - lo, self.rows_per_board, -1)[:, :, :self.L["n_live"]]
+                for idx in _decision_row_groups(self.st, self.local_rows):
+                    rows[:, idx] = _sum_to_one(rows[:, idx], 1)
+            if lo == 0:  # the trunk's rows, then its reach: the sweeps read the opponent's reach at the chance node
+                self.bufs.avg[:nts].copy_(tab[:nts])
+                if normalise:
+                    for fs, A in _trunk_decisions(self.ft1, self.chance_node):
+                        self.bufs.avg[fs:fs + A, :R] = _sum_to_one(self.bufs.avg[fs:fs + A, :R], 0)
+                self._reach_trunk(self.bufs, 3, -1, -1, [nat.STRAT_AVG_F32, nat.STRAT_AVG_F32], 0, 0)
+            t0 = tick("table build", t0)
+            yield lo, hi, t0
+            del pt
+
+    def model_reach(self, agent, tables):
+        """restricted Nash response: for every {seat s: float32 [n_boards_total * n_sd, 1088] table}, the reach of `agent`
+        playing seat 1 - s at the showdown terminals of every board of the spec (prl_board_sweep, p1_only with rnr_reach),
+        in one pass over the agent's answers; returns the agent's trunk reach rows (float32 [2, nodes, ld], a copy)"""
+        n_sd = sum(1 for k in self.st["kind"][:self.st["n_local"]] if k == nat.KIND_SHOWDOWN)
+        with torch.cuda.device(self.device):
+            for lo, hi, _ in self._chunks(agent, lambda key, t0: t0, normalise=True):
+                for seat, F in tables.items():
+                    g = nat.PrlBoardGame.from_buffer_copy(self.g)
+                    g.rnr_reach, g.rnr_p = F[lo * n_sd].data_ptr(), 1.0
+                    nat.call("prl_board_sweep", C.byref(g), seat, 0, SRC_AVG, SRC_AVG,
+                             self._trunk_reach_row(self.bufs, 1 - seat), 0, 0, nat.ALGO_CFR_PLUS, 0.0, 1, _stream(self.device))
+            return self.bufs.reach.clone()
+
     def evaluate(self, agent, profile=False):
         """exploitability of each seat in chips, numpy float64 [2] (the analogue of PublicTree's root.exploitability).
         profile=True synchronises between the phases and leaves their wall times (s) in self.times."""
         import time
-        dev, R, s = self.device, self.R, self.spec
+        dev = self.device
         times = {"agent query": 0.0, "table build": 0.0, "sweeps": 0.0}
         modes = [nat.STRAT_AVG_F32, nat.STRAT_AVG_F32]
 
@@ -701,28 +923,11 @@ class BoardPolicyEvaluator(_BoardEngine):
 
         with torch.cuda.device(dev):
             self.w_acc.zero_()
-            nts = self.n_trunk_slots
-            for lo in range(0, self.n_boards_total, self.chunk):
-                hi = min(lo + self.chunk, self.n_boards_total)
-                t0 = time.perf_counter()
-                pt = self._chunk_tree(lo, hi)
-                ft = pt.flat
-                tab = self.nat_tab[:ft.n_slots]
-                got = pt.agent_strategy_table(agent, out=tab)
-                if not isinstance(got, torch.Tensor):  # answered node by node on the host
-                    tab[:, :R].copy_(torch.from_numpy(np.ascontiguousarray(got, np.float32)))
-                t0 = tick("agent query", t0)
-                self._load_boards(s.boards[lo:hi], s.board_prob[lo:hi], s.board_mult[lo:hi])
-                self._board_permute(self.rows, tab, 0, ft)
-                if lo == 0:  # the trunk's rows, then its reach: the sweeps read the opponent's reach at the chance node
-                    self.bufs.avg[:nts].copy_(tab[:nts])
-                    self._reach_trunk(self.bufs, 3, -1, -1, modes, 0, 0)
-                t0 = tick("table build", t0)
+            for lo, hi, t0 in self._chunks(agent, tick):
                 for p in (0, 1):  # prl_board_sweep zeroes the arrays it writes at every launch: accumulate outside
                     self._board_sweep(self.bufs, p, True, SRC_AVG, SRC_AVG, 0, 0, nat.ALGO_CFR_PLUS)
                     self.w_acc[2 * p:2 * p + 2] += self.w_total[2 * p:2 * p + 2]
                 tick("sweeps", t0)
-                del pt
             t0 = time.perf_counter()
             self.w_total.copy_(self.w_acc)
             self._board_trunk(self.bufs, modes, True, -1, 0, 0, nat.ALGO_CFR_PLUS)
@@ -759,8 +964,7 @@ class BoardPolicyTables:
         s.flush_average()
         avg = s.alg.average(s.iter_counter)
         nb, rpb, st = s.n_boards, s.rows_per_board, s.st
-        groups = [[s.local_rows[c][0] for c in range(st["first_child"][d], st["first_child"][d] + st["n_children"][d])]
-                  for d in _decision_locals(st)]
+        groups = _decision_row_groups(st, s.local_rows)
         with torch.cuda.device(s.device):
             if avg == algorithm.AVERAGE:
                 rows = s.avg.clone()

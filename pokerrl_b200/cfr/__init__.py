@@ -1,4 +1,5 @@
 from pokerrl_b200.cfr.DiscountedCFR import DiscountedCFR
 from pokerrl_b200.cfr.PredictiveCFRPlus import PredictiveCFRPlus
+from pokerrl_b200.cfr.RestrictedNashResponse import RestrictedNashResponse
 
-__all__ = ["DiscountedCFR", "PredictiveCFRPlus"]
+__all__ = ["DiscountedCFR", "PredictiveCFRPlus", "RestrictedNashResponse"]

@@ -319,10 +319,19 @@ __device__ __forceinline__ void st_stream(float* p, float v) { __stcs(p, v); }
 // regret rows and the own prediction rows (in the registers the paired form gives its average rows), takes the strategy from
 // the predictions and writes R = max(d + R, 0), then Q = max(R + d, 0).  The average is DEFER's reach-weighted sum (defer_w =
 // w_t).  PCFR+'s evaluation and flush run the EVAL / P1ONLY forms on a copy of the descriptor whose `regret` is `pred`.
-template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true, bool PRED = false>
+// RNR (restricted Nash response; Johanson, Zinkevich & Bowling, NIPS 2007): the opponent is a mixture of a fixed model
+// (probability G.rnr_p) and a free strategy.  The values of seat P are linear in the opponent's reach, so the mixture only
+// changes what P1 writes into S: kRnrMix adds G.rnr_p times the model's showdown reach G.rnr_reach[j][v] (trunk reach and deal
+// included; the caller scales trunk_reach_opp by 1 - rnr_p) and takes the fold terminals' share through SH::fold_coef, which
+// holds for any opponent whose rows sum to one.  CFR+ update forms (the exploiter's update) and the evaluation form (the
+// exploitation of the model, with rnr_p = 1 and a zero trunk_reach_opp).  kRnrOut: P1 only, the opponent's strategy = the rows
+// of `avg` as they are (the model), its showdown reach written to G.rnr_reach instead of S.
+constexpr int kRnrMix = 1, kRnrOut = 2;
+template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true, bool PRED = false, int RNR = 0>
 __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArgs a) {
-    static_assert(!(EVAL && DEFER) && (!P1ONLY || DEFER) && (AVG || (!EVAL && !DEFER)), "variants");
+    static_assert(!(EVAL && DEFER) && (!P1ONLY || DEFER || RNR == kRnrOut) && (AVG || (!EVAL && !DEFER)), "variants");
     static_assert(!PRED || (DEFER && !P1ONLY), "PRED is an update form of the DEFER family");
+    static_assert(RNR == 0 || (!DEFER && !PRED && (RNR == kRnrOut) == P1ONLY && (RNR == kRnrMix || !EVAL)), "RNR forms");
     using M = SweepSmem<SH>;
     constexpr int NSD = SH::n_sd, NF = SH::n_fold;
     extern __shared__ __align__(128) unsigned char smem[];
@@ -350,9 +359,10 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
     constexpr size_t kBoardFloats = (size_t)ROWS * kLdb;
     const unsigned char* blob_g = reinterpret_cast<const unsigned char*>(G.tables);
     // tables the two seats' strategies come from (evaluation: regret matching of `regret` or the rows of `avg`)
-    const float* tab_opp = PRED ? G.pred : (EVAL && a.src_opp >= 1) ? G.avg : G.regret;
+    const float* tab_opp = PRED ? G.pred : (RNR == kRnrOut || (EVAL && a.src_opp >= 1)) ? G.avg : G.regret;
     const float* tab_own = (EVAL && a.src_own >= 1) ? G.avg : G.regret;
-    const int asis_opp = (EVAL && a.src_opp == 1) ? 1 : 0, asis_own = (EVAL && a.src_own == 1) ? 1 : 0;
+    const int asis_opp = (RNR == kRnrOut || (EVAL && a.src_opp == 1)) ? 1 : 0, asis_own = (EVAL && a.src_own == 1) ? 1 : 0;
+    constexpr size_t kRnrFloats = (size_t)SH::n_sd * kLdb;  // G.rnr_reach per board
     const bool do_avg = !EVAL && !DEFER && AVG && a.iter >= a.delay;
     const bool pair = do_avg && a.pair;
     const bool defer_now = DEFER && a.defer_w != 0.0f;
@@ -384,6 +394,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
         bulk_prefetch_l2(tab_own + (size_t)jj * kBoardFloats + (size_t)OWN0 * kLdb, NOWN * kLdb * 4);
         if (read_avg) bulk_prefetch_l2(G.avg + (size_t)jj * kBoardFloats + (size_t)OWN0 * kLdb, NOWN * kLdb * 4);
         if (defer_now) bulk_prefetch_l2(G.avg + (size_t)jj * kBoardFloats + (size_t)OPP0 * kLdb, NOPP * kLdb * 4);
+        if constexpr (RNR == kRnrMix) bulk_prefetch_l2(G.rnr_reach + (size_t)jj * kRnrFloats, kRnrFloats * 4);
     };
     // Update forms: each stream one phase ahead of its first use, so that a CTA holds about one board's rows in L2, not two -
     // two boards of the paired form (264 CTAs x (2 x 91 KB read + 61 KB stored)) overflow the 50 MB L2 of an H100, and rows
@@ -394,6 +405,7 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
     auto prefetch_opp = [&](int jj) {
         bulk_prefetch_l2(tab_opp + (size_t)jj * kBoardFloats + (size_t)OPP0 * kLdb, NOPP * kLdb * 4);
         if (defer_now) bulk_prefetch_l2(G.avg + (size_t)jj * kBoardFloats + (size_t)OPP0 * kLdb, NOPP * kLdb * 4);
+        if constexpr (RNR == kRnrMix) bulk_prefetch_l2(G.rnr_reach + (size_t)jj * kRnrFloats, kRnrFloats * 4);  // P1 only reads them
     };
     // ... rows first read in P3: this unit's own rows (paired form: and the average rows), prefetched at B1 to load behind P2
     auto prefetch_own = [&](int jj) {
@@ -452,6 +464,11 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
             if (i < kLive) {
                 float x[SH::N];
                 x[0] = x0k * prob;  // the deal (StrategyFiller.py:137-140); blocked hands are not stored at all
+                float fm[RNR == kRnrMix ? NSD : 1];  // kRnrMix: the model's showdown reach of this hand
+                if constexpr (RNR == kRnrMix) {
+#pragma unroll
+                    for (int v = 0; v < NSD; ++v) fm[v] = ld_stream(G.rnr_reach + (size_t)j * kRnrFloats + (size_t)v * kLdb + i);
+                }
                 static_for<0, SH::N>([&](auto I) {
                     constexpr int n = decltype(I)::value;
                     constexpr int A = SH::n_children(n);
@@ -480,8 +497,20 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
                             for (int c = 0; c < A; ++c) x[fc + c] = x[n];
                         }
                     } else if constexpr (SH::kind(n) == 4) {
-                        S[SH::vec_index(n) * kLdb + i] = x[n];
-                    } else {
+                        constexpr int v = SH::vec_index(n);
+                        if constexpr (RNR == kRnrOut) st_stream(G.rnr_reach + (size_t)j * kRnrFloats + (size_t)v * kLdb + i, x[n]);
+                        else if constexpr (RNR == kRnrMix) S[v * kLdb + i] = __fmaf_rn(G.rnr_p, fm[v], x[n]);
+                        else S[v * kLdb + i] = x[n];
+                    } else if constexpr (RNR == kRnrMix) {  // the model's fold reach: x_fold[f] = sum_v fold_coef * x_sd[v]
+                        constexpr int f = SH::vec_index(n);
+                        float m = 0.0f;
+                        static_for<0, NSD>([&](auto V) {
+                            constexpr int cf = SH::fold_coef(P, f, decltype(V)::value);
+                            if constexpr (cf > 0) m = __fadd_rn(m, fm[decltype(V)::value]);
+                            else if constexpr (cf < 0) m = __fsub_rn(m, fm[decltype(V)::value]);
+                        });
+                        S[(NSD + f) * kLdb + i] = __fmaf_rn(G.rnr_p, m, x[n]);
+                    } else if constexpr (RNR != kRnrOut) {
                         S[(NSD + SH::vec_index(n)) * kLdb + i] = x[n];
                     }
                 });
@@ -1090,7 +1119,10 @@ __device__ __forceinline__ float trunk_sigma(const prl_trunk_t& t, int src, int 
 // into w_scratch; the caller has placed a cross-rank barrier between the sweep kernels and this launch.
 // PRED (PCFR+ update): regrets max(d + R, 0), stored strategy = regret matching of max(R + d, 0), average += s * reach * w_t
 // with w_t = disc[2] (no discount)
-template <bool EVAL, bool PRED = false>
+// RNR (restricted Nash response, t.reach_model): update form, the opponent's reach at the fold terminals is the mixture
+// (1 - rnr_p) * free + rnr_p * model; evaluation form, out_expl[2 + p] / out_expl[4 + p] = the root value / best-response
+// value of seat p as well
+template <bool EVAL, bool PRED = false, bool RNR = false>
 __global__ void __launch_bounds__(kTrunkThreads) trunk_kernel(const prl_trunk_t t, const long long* __restrict__ w_total,
                                                               const long long* const* __restrict__ peers, int n_peers,
                                                               long long peer_offset, long long* __restrict__ w_scratch,
@@ -1136,7 +1168,9 @@ __global__ void __launch_bounds__(kTrunkThreads) trunk_kernel(const prl_trunk_t 
             __syncthreads();
             float part = 0.0f;
             for (int h = tid; h < kRange; h += kTrunkThreads) {
-                const float r = rg[h];
+                float r = rg[h];
+                if constexpr (RNR && !EVAL)
+                    r = __fmaf_rn(t.rnr_p, t.reach_model[((size_t)(1 - p) * N + n) * ld + h], __fmul_rn(1.0f - t.rnr_p, r));
                 ro[h] = r;
                 part += r;
             }
@@ -1166,7 +1200,7 @@ __global__ void __launch_bounds__(kTrunkThreads) trunk_kernel(const prl_trunk_t 
     }
     __syncthreads();
     // 3. decision nodes bottom-up, per hand (children have larger ids); 4. regrets / matching / average; 5. reach of seat p
-    double ex[2] = {0.0, 0.0};
+    double ex[2] = {0.0, 0.0}, root_ev[2] = {0.0, 0.0}, root_br[2] = {0.0, 0.0};
     for (int h = tid; h < kRange; h += kTrunkThreads) {
         for (int n = t.n_nodes - 1; n >= 0; --n) {
             const int k = t.kind[n];
@@ -1224,8 +1258,14 @@ __global__ void __launch_bounds__(kTrunkThreads) trunk_kernel(const prl_trunk_t 
         }
         if (EVAL) {
             for (int p = 0; p < 2; ++p)  // ValueFiller.py:95-101 at the root
+            {
                 ex[p] += (double)t.reach[((size_t)p * N) * ld + h] *
                          ((double)t.ev_br[((size_t)p * N) * ld + h] - (double)t.ev[((size_t)p * N) * ld + h]);
+                if constexpr (RNR) {
+                    root_ev[p] += (double)t.reach[((size_t)p * N) * ld + h] * (double)t.ev[((size_t)p * N) * ld + h];
+                    root_br[p] += (double)t.reach[((size_t)p * N) * ld + h] * (double)t.ev_br[((size_t)p * N) * ld + h];
+                }
+            }
         } else {
             const int p = p_upd;
             float* rp = t.reach + (size_t)p * N * ld;
@@ -1260,6 +1300,20 @@ __global__ void __launch_bounds__(kTrunkThreads) trunk_kernel(const prl_trunk_t 
                 double s = 0.0;
                 for (int w = 0; w < kTrunkThreads / 32; ++w) s += dred[w];
                 out_expl[p] = (float)s;
+            }
+        }
+        if constexpr (RNR) {
+            for (int q = 0; q < 4; ++q) {
+                double v = (q < 2) ? root_ev[q] : root_br[q - 2];
+                for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+                __syncthreads();
+                if (lane == 0) dred[warp] = v;
+                __syncthreads();
+                if (tid == 0) {
+                    double s = 0.0;
+                    for (int w = 0; w < kTrunkThreads / 32; ++w) s += dred[w];
+                    out_expl[2 + q] = (float)s;
+                }
             }
         }
     }
@@ -1306,9 +1360,9 @@ int default_grid() {
     return cached[dev];
 }
 
-template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true, bool PRED = false>
+template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true, bool PRED = false, int RNR = 0>
 int launch_sweep(const SweepArgs& a, int grid, cudaStream_t s) {
-    auto kern = board_sweep_kernel<SH, P, EVAL, DEFER, P1ONLY, AVG, PRED>;
+    auto kern = board_sweep_kernel<SH, P, EVAL, DEFER, P1ONLY, AVG, PRED, RNR>;
     constexpr int kSmemBytes = SweepSmem<SH>::kSmemBytes;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);  // per device: set every time
     if (e != cudaSuccess) return prl::check(e, "prl_board_sweep: shared memory opt-in");
@@ -1368,7 +1422,12 @@ static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, 
     const bool pred = algo == PRL_ALGO_PCFR_PLUS;
     if (pred && !g->pred) return prl::fail("prl_board_sweep: PCFR+ needs the prediction table g->pred");
     const bool defer = !eval && algo != PRL_ALGO_CFR_PLUS;
-    if (p1_only && !defer) return prl::fail("prl_board_sweep: p1_only is the average flush of Vanilla / Linear CFR");
+    const bool rnr = g->rnr_reach != nullptr;
+    if (rnr && algo != PRL_ALGO_CFR_PLUS) return prl::fail("prl_board_sweep: the restricted Nash response is a CFR+ form");
+    if (rnr && !(g->rnr_p >= 0.0f && g->rnr_p <= 1.0f)) return prl::fail("prl_board_sweep: rnr_p must be in [0, 1]");
+    if (p1_only && !defer && !rnr)
+        return prl::fail("prl_board_sweep: p1_only is the average flush of Vanilla / Linear CFR or the model reach of a restricted "
+                         "Nash response");
     const int layout_ok = with_shape(g, [&](auto sh) { return layout_matches<decltype(sh)>(g) ? 1 : 0; });
     if (layout_ok == kNoShape) return prl::fail("prl_board_sweep: the post-deal subtree has no compiled shape");
     if (g->n_range != kRange || g->n_deck != kDeck) return prl::fail("prl_board_sweep: 52-card deck / 1326 hands only");
@@ -1406,6 +1465,8 @@ static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, 
     if (p1_only) {
         const int rc1 = with_shape(g, [&](auto sh) {
             using SH = decltype(sh);
+            if (rnr) return (p == 0) ? launch_sweep<SH, 0, false, false, true, false, false, kRnrOut>(a, grid, s)
+                                     : launch_sweep<SH, 1, false, false, true, false, false, kRnrOut>(a, grid, s);
             return (p == 0) ? launch_sweep<SH, 0, false, true, true>(a, grid, s) : launch_sweep<SH, 1, false, true, true>(a, grid, s);
         });
         return rc1 ? rc1 : prl::check(cudaGetLastError(), "prl_board_sweep(flush)");
@@ -1416,7 +1477,13 @@ static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, 
     }
     const int rc = with_shape(g, [&](auto sh) {
         using SH = decltype(sh);
+        if (eval && rnr) return (p == 0) ? launch_sweep<SH, 0, true, false, false, true, false, kRnrMix>(a, grid, s)
+                                         : launch_sweep<SH, 1, true, false, false, true, false, kRnrMix>(a, grid, s);
         if (eval) return (p == 0) ? launch_sweep<SH, 0, true>(a, grid, s) : launch_sweep<SH, 1, true>(a, grid, s);
+        if (rnr && step) return (p == 0) ? launch_sweep<SH, 0, false, false, false, true, false, kRnrMix>(a, grid, s)
+                                         : launch_sweep<SH, 1, false, false, false, true, false, kRnrMix>(a, grid, s);
+        if (rnr) return (p == 0) ? launch_sweep<SH, 0, false, false, false, false, false, kRnrMix>(a, grid, s)
+                                 : launch_sweep<SH, 1, false, false, false, false, false, kRnrMix>(a, grid, s);
         if (pred) return (p == 0) ? launch_sweep<SH, 0, false, true, false, true, true>(a, grid, s)
                                   : launch_sweep<SH, 1, false, true, false, true, true>(a, grid, s);
         if (defer) return (p == 0) ? launch_sweep<SH, 0, false, true>(a, grid, s) : launch_sweep<SH, 1, false, true>(a, grid, s);
@@ -1537,7 +1604,14 @@ extern "C" int prl_board_trunk(const prl_board_game_t* g, const prl_trunk_t* t, 
     if (peers && (n_peers < 1 || !w_scratch)) return prl::fail("prl_board_trunk: peer sum needs n_peers >= 1 and w_scratch");
     const long long* const* pp = reinterpret_cast<const long long* const*>(peers);
     long long* ws = reinterpret_cast<long long*>(w_scratch);
-    if (eval)
+    const bool rnr = t->reach_model != nullptr;
+    if (rnr && (algo != PRL_ALGO_CFR_PLUS || !(t->rnr_p >= 0.0f && t->rnr_p <= 1.0f)))
+        return prl::fail("prl_board_trunk: the restricted Nash response is a CFR+ form with rnr_p in [0, 1]");
+    if (rnr)
+        (eval ? trunk_kernel<true, false, true> : trunk_kernel<false, false, true>)<<<1, kTrunkThreads, 0, (cudaStream_t)stream>>>(
+            *t, w, pp, n_peers, (long long)peer_offset, ws, sym_perm, n_sym, inv_scale, eval ? -1 : p, iter, delay, m_old, m_new, algo,
+            rw, disc, out_expl);
+    else if (eval)
         trunk_kernel<true><<<1, kTrunkThreads, 0, (cudaStream_t)stream>>>(*t, w, pp, n_peers, (long long)peer_offset, ws, sym_perm, n_sym,
                                                                        inv_scale, -1, iter, delay, m_old, m_new, algo, rw, disc, out_expl);
     else if (pred)
