@@ -10,7 +10,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "_build", "libcfr2_oracle.so")
 _lib = None
-ALGOS = {"VanillaCFR": 0, "CFRPlus": 1, "LinearCFR": 2}
+ALGOS = {"VanillaCFR": 0, "CFRPlus": 1, "LinearCFR": 2, "DCFR": 3, "PCFRPlus": 4}  # include/pokerrl_b200.h PRL_ALGO_*
 
 
 class Orc2(C.Structure):
@@ -19,7 +19,8 @@ class Orc2(C.Structure):
                [(k, C.c_void_p) for k in ("level_start", "parent", "first_child", "n_children", "slot", "board", "kind",
                                           "acted_last", "pot", "hand_cards", "board_ranks", "board_blocked", "board_prob",
                                           "board_mult", "sym_perm", "board_order", "board_nlive")] + \
-               [("K", C.c_double)] + [(k, C.c_void_p) for k in ("reach", "ev", "ev_br", "regret", "strat", "avg")]
+               [("K", C.c_double)] + [(k, C.c_void_p) for k in ("reach", "ev", "ev_br", "regret", "strat", "avg", "pred")] + \
+               [(k, C.c_double) for k in ("fa", "fb", "fw")]
 
 
 def build():
@@ -39,6 +40,7 @@ def lib():
         L.orc2_reach.argtypes = [tp, C.c_void_p]
         L.orc2_values.argtypes = [tp, C.c_void_p, C.c_int, C.c_int]
         L.orc2_values_levels.argtypes = [tp, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]
+        L.orc2_match.argtypes = [tp, C.c_void_p]
         L.orc2_regret_match.argtypes = [tp]
         L.orc2_exploitability.argtypes = [tp, C.c_void_p]
         L.orc2_regret_update.argtypes = [tp, C.c_int, C.c_int, C.c_int]
@@ -47,12 +49,23 @@ def lib():
         L.orc2_fold_row.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p]
         L.orc2_showdown_row.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                         C.c_double, C.c_void_p]
-        for f in ("orc2_prepare", "orc2_fill_uniform", "orc2_reach", "orc2_values", "orc2_values_levels", "orc2_regret_match",
+        for f in ("orc2_prepare", "orc2_fill_uniform", "orc2_reach", "orc2_values", "orc2_values_levels", "orc2_match",
+                  "orc2_regret_match",
                   "orc2_exploitability",
                   "orc2_regret_update", "orc2_avg_update", "orc2_average_strategy", "orc2_fold_row", "orc2_showdown_row"):
             getattr(L, f).restype = None
         _lib = L
     return _lib
+
+
+def set_factors(t, algo, it, dcfr_params=None, pcfr_gamma=2.0):
+    """the factors of iteration counter `it` into the Orc2 struct t before a DCFR / PCFR+ update: the float32 row
+    {a_t, b_t, w_t} of pokerrl_b200.dcfr.factors (PCFR+: of pcfr_params(gamma)), the numbers the kernels read"""
+    if algo not in ("DCFR", "PCFRPlus"):
+        return
+    from pokerrl_b200 import dcfr
+    params = (dcfr.DEFAULT if dcfr_params is None else dcfr_params) if algo == "DCFR" else dcfr.pcfr_params(pcfr_gamma)
+    t.fa, t.fb, t.fw = (float(x) for x in dcfr.factors(*params, it + 1)[it])
 
 
 def terminal_rows(hand_cards, ranks, reach, K, n_deck=52):
@@ -75,9 +88,11 @@ def terminal_rows(hand_cards, ranks, reach, K, n_deck=52):
 class Oracle2CSolver:
     """ft: FlatTree of a two-card game; board_ranks int32 [n_boards_total, R] in global board id order (-1 = blocked)."""
 
-    def __init__(self, ft, board_ranks, algo="CFRPlus", delay=0, ev_normalizer=None, n_threads=None, lean=False):
+    def __init__(self, ft, board_ranks, algo="CFRPlus", delay=0, ev_normalizer=None, n_threads=None, lean=False,
+                 dcfr_params=None, pcfr_gamma=2.0):
         self.ft, self.algo_name, self.algo = ft, algo, ALGOS[algo]
         self.delay = delay if algo == "CFRPlus" else 0
+        self.dcfr_params, self.pcfr_gamma = dcfr_params, pcfr_gamma
         self.lean = bool(lean)  # True: value passes compute only what the half-iteration needs (the GPU's schedule)
         self.ev_normalizer = ft.game_cls.EV_NORMALIZER if ev_normalizer is None else ev_normalizer
         L = self.L = lib()
@@ -106,6 +121,8 @@ class Oracle2CSolver:
         self.reach, self.ev, self.ev_br = (np.zeros((N, 2, R)) for _ in range(3))
         self.regret, self.strat, self.avg = (np.zeros((S, R)) for _ in range(3))
         self._avg_norm = np.zeros((S, R))
+        # PCFR+: the predictions; the strategy is regret matching of these rows
+        self.pred = np.zeros((S, R)) if algo == "PCFRPlus" else None
         t = Orc2()
         t.n_nodes, t.n_levels, t.n_slots, t.R = N, ft.n_levels, S, R
         t.n_deck, t.n_boards, t.n_sym = rules.N_CARDS_IN_DECK, nb, 0 if sp is None else sp.shape[0]
@@ -115,15 +132,22 @@ class Oracle2CSolver:
         t.K = comb(t.n_deck, n_hole) / comb(t.n_deck - n_hole, n_hole)
         for k in ("reach", "ev", "ev_br", "regret", "strat", "avg"):
             setattr(t, k, getattr(self, k).ctypes.data)
+        t.pred = None if self.pred is None else self.pred.ctypes.data
         self.t = t
         L.orc2_prepare(C.byref(t))
         self.reset()
 
     def reset(self):
         self.iter_counter = 0
-        for a in (self.regret, self.strat, self.avg):
+        for a in (self.regret, self.strat, self.avg) + (() if self.pred is None else (self.pred,)):
             a[:] = 0
         self.L.orc2_fill_uniform(C.byref(self.t))
+        self.L.orc2_reach(C.byref(self.t), self.strat.ctypes.data)
+
+    def match(self):
+        """strategy = regret matching of the regret rows (PCFR+: of the predictions), reach refreshed: after the caller
+        set the tables"""
+        self.L.orc2_regret_match(C.byref(self.t))
         self.L.orc2_reach(C.byref(self.t), self.strat.ctypes.data)
 
     def compute_ev(self, mask=3, with_br=True):
@@ -139,6 +163,7 @@ class Oracle2CSolver:
             self.L.orc2_values(t, self.strat.ctypes.data, 1 << p, 0)
         else:
             self.L.orc2_values(t, self.strat.ctypes.data, 3, 1)
+        set_factors(self.t, self.algo_name, self.iter_counter, self.dcfr_params, self.pcfr_gamma)
         self.L.orc2_regret_update(t, p, self.algo, self.iter_counter)
         self.L.orc2_reach(t, self.strat.ctypes.data)
         self.L.orc2_avg_update(t, p, self.algo, self.iter_counter, self.delay)
@@ -153,6 +178,7 @@ class Oracle2CSolver:
         return float(sum(expl[p] * self.ev_normalizer for p in range(2)) / 2)
 
     def exploitability_current(self):
+        """of the current strategy: regret matching of the regrets (PCFR+: of the predictions), as the updates leave it"""
         return self._metric(self.compute_ev())
 
     def exploitability_average(self):

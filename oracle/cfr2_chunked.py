@@ -1,5 +1,6 @@
 """Float64 results of a two-card game with ONE chance layer, computed a chunk of boards at a time (oracle/cfr2_oracle.c).
-TEST INFRASTRUCTURE ONLY (tests/test_oracle_cfr2_chunked.py, tests/test_gpu_board_full_game.py).
+TEST INFRASTRUCTURE ONLY (tests/test_oracle_cfr2_chunked.py, tests/test_gpu_board_full_game.py,
+tests/test_gpu_board_full_game_dcfr_pcfr.py).
 
 The full Flop5Holdem game (134 459 board classes) does not fit the monolithic oracle: each of its float64 node vectors would
 take ~45 GB.  But everything below the chance node is per board, and the chance node's row is linear in its children
@@ -12,8 +13,8 @@ take ~45 GB.  But everything below the chance node is per board, and the chance 
   3. for an update, every chunk is swept again with the updated trunk rows in place: its post-update board rows go to a
      callback, so nothing full-size is ever held.
 
-`SyntheticProfile` is the deterministic input both sides load: regrets and average rows from an integer hash of (board
-class, local node, hand), in float32 values that are exact in float64."""
+`SyntheticProfile` is the deterministic input both sides load: regrets and average rows (PCFR+: and predictions) from an
+integer hash of (board class, local node, hand), in float32 values that are exact in float64."""
 import ctypes as C
 
 import numpy as np
@@ -23,6 +24,7 @@ from pokerrl_b200.game.holdem_boards import BoardSpec
 
 _M32 = 0xFFFFFFFF
 _TRUNK_KEY = 0x7FFFFFFF
+_PRED_SALT = 0x5BD1E995
 
 
 def _mix(x):
@@ -58,14 +60,17 @@ class SyntheticProfile:
     (1/4) or a positive regret of 1 .. 2^20 units; per (decision node, hand) a second hash makes 1/8 of the hands all <= 0
     (regret matching falls back to uniform) and 1/8 pure (one positive action).  The average rows are integer weights
     0 .. 255 (1/8 zero) normalised per hand (uniform where all are 0).  Units: regret 2^(regret_exp - 20), average
-    2^avg_exp (CFR+: 0, a strategy; Vanilla / Linear CFR: reach-weighted sums of the size of one iteration's contribution),
-    each as (trunk, board) exponents, so that one update's increment is not lost in the inputs."""
+    2^avg_exp (CFR+: 0, a strategy; Vanilla / Linear CFR, DCFR, PCFR+: reach-weighted sums of the size of one iteration's
+    contribution), each as (trunk, board) exponents, so that one update's increment is not lost in the inputs.
+    pcfr=True (PCFR+): the regrets are clipped at 0, and prediction rows come from a third hash of the same keys by the
+    regrets' construction, clipped at 0 (exact zeros, all-zero hands whose matching is uniform, pure hands), in the regrets'
+    units; the row methods then return (regret, avg, pred)."""
 
-    def __init__(self, ft, seed=1, regret_exp=(0, 0), avg_exp=(0, 0)):
+    def __init__(self, ft, seed=1, regret_exp=(0, 0), avg_exp=(0, 0), pcfr=False):
         st = ft.board_subtree()
         self.R = ft.R
         self.seed = int(seed) & _M32
-        self.regret_exp, self.avg_exp = regret_exp, avg_exp
+        self.regret_exp, self.avg_exp, self.pcfr = regret_exp, avg_exp, bool(pcfr)
         self.rows = decision_rows(st)
         par = [st["parent"][c] for c in self.rows]
         self._board = self._meta(self.rows, par, [c - st["first_child"][p] for c, p in zip(self.rows, par)],
@@ -85,6 +90,18 @@ class SyntheticProfile:
                     n_act=np.array(n_act, np.int64), group=np.array([groups[p] for p in parent], np.int64),
                     n_groups=len(groups))
 
+    @staticmethod
+    def _signed(e, g, meta, t):
+        """integer regrets (units) from the entry hashes e and the (decision node, hand) hashes g"""
+        import torch
+        mag = (e & 0xFFFFF) + 1
+        sel = (e >> 20) & 15
+        val = torch.where(sel < 2, torch.zeros_like(mag), torch.where(sel < 6, -mag, mag))
+        mode = g & 7
+        chosen = ((g >> 3) % t(meta["n_act"])[None, :, None]) == t(meta["action"])[None, :, None]
+        val = torch.where(mode == 0, -val.abs(), val)
+        return torch.where(mode == 1, torch.where(chosen, mag, -val.abs()), val)
+
     def _rows(self, keys, meta, part, device):
         import torch
         t = lambda a: torch.as_tensor(a, dtype=torch.int64, device=device)  # noqa: E731
@@ -93,14 +110,11 @@ class SyntheticProfile:
         kg = _mix(kc ^ (((t(meta["parent"]) + 32) * 0x9E3779B1) & _M32)[None, :])[..., None]
         h = torch.arange(self.R, dtype=torch.int64, device=device)[None, None, :]
         e, g = _mix(ke ^ h), _mix(kg ^ h)
-        mag = (e & 0xFFFFF) + 1
-        sel = (e >> 20) & 15
-        val = torch.where(sel < 2, torch.zeros_like(mag), torch.where(sel < 6, -mag, mag))
-        mode = g & 7
-        chosen = ((g >> 3) % t(meta["n_act"])[None, :, None]) == t(meta["action"])[None, :, None]
-        val = torch.where(mode == 0, -val.abs(), val)
-        val = torch.where(mode == 1, torch.where(chosen, mag, -val.abs()), val)
-        regret = (val.to(torch.float64) * 2.0 ** (self.regret_exp[part] - 20)).to(torch.float32)
+        val = self._signed(e, g, meta, t)
+        if self.pcfr:
+            val = val.clamp(min=0)
+        unit = 2.0 ** (self.regret_exp[part] - 20)
+        regret = (val.to(torch.float64) * unit).to(torch.float32)
         z = (e >> 24) & 0xFF
         w = torch.where(z < 32, torch.zeros_like(z), z).to(torch.float64)
         gid = t(meta["group"])
@@ -108,25 +122,28 @@ class SyntheticProfile:
         tot = tot[:, gid]
         avg = torch.where(tot > 0, w / torch.where(tot > 0, tot, torch.ones_like(tot)), 1.0 / t(meta["n_act"])[None, :, None])
         avg = (avg.to(torch.float32).to(torch.float64) * 2.0 ** self.avg_exp[part]).to(torch.float32)
-        return regret, avg
+        if not self.pcfr:
+            return regret, avg
+        e3, g3 = _mix(_mix(ke ^ _PRED_SALT) ^ h), _mix(_mix(kg ^ _PRED_SALT) ^ h)
+        pred = (self._signed(e3, g3, meta, t).clamp(min=0).to(torch.float64) * unit).to(torch.float32)
+        return regret, avg, pred
 
     def board_rows(self, classes, device="cpu"):
-        """(regret, avg) float32 [len(classes), len(self.rows), R] of the given global board classes"""
+        """(regret, avg[, pred]) float32 [len(classes), len(self.rows), R] of the given global board classes"""
         return self._rows(np.asarray(classes, np.int64), self._board, 1, device)
 
     def trunk_rows(self, device="cpu"):
-        """(regret, avg) float32 [n_trunk_slots, R]"""
-        r, a = self._rows(np.array([_TRUNK_KEY], np.int64), self._trunk, 0, device)
-        return r[0], a[0]
+        """(regret, avg[, pred]) float32 [n_trunk_slots, R]"""
+        return tuple(x[0] for x in self._rows(np.array([_TRUNK_KEY], np.int64), self._trunk, 0, device))
 
     def tables(self, ft, first_class, device="cpu"):
-        """(regret, avg) float64 [ft.n_slots, R] over a flat tree whose boards are the classes first_class, first_class + 1, ...
-        (device: where the hash runs; integer arithmetic, so any device gives the same bits)"""
+        """(regret, avg[, pred]) float64 [ft.n_slots, R] over a flat tree whose boards are the classes first_class,
+        first_class + 1, ... (device: where the hash runs; integer arithmetic, so any device gives the same bits)"""
         nb = ft.board_spec.boards.shape[0]
         out = []
         tr, br = self.trunk_rows(device), self.board_rows(np.arange(first_class, first_class + nb), device)
         slots = board_slots(ft, self.rows)
-        for k in range(2):
+        for k in range(len(tr)):
             tab = np.zeros((ft.n_slots, self.R))
             tab[:self.n_trunk_slots] = tr[k].cpu().numpy()
             tab[slots.ravel()] = br[k].cpu().numpy().reshape(-1, self.R)
@@ -143,11 +160,14 @@ def spec_slice(spec, lo, hi):
 class ChunkedOracle:
     """tree_fn(BoardSpec) -> FlatTree of the game; ranks: int32 [n_boards, R] of spec.boards (-1: the hand holds a board
     card); tables(ft, first_class, key) -> (regret, avg) float64 [ft.n_slots, R] for the chunk tree ft of the classes
-    first_class, ... (`key` names one set of tables; runs that share one computation of values must share the regrets)."""
+    first_class, ..., and (regret, avg, pred) for a PCFR+ key (`key` names one set of tables; runs that share one
+    computation of values must share the strategy: the regrets, or PCFR+'s predictions).  dcfr_params / pcfr_gamma: the
+    factors of DCFR / PCFR+ runs (pokerrl_b200.dcfr)."""
 
-    def __init__(self, tree_fn, spec, ranks, tables, chunk=2048, n_threads=None):
+    def __init__(self, tree_fn, spec, ranks, tables, chunk=2048, n_threads=None, dcfr_params=None, pcfr_gamma=2.0):
         self.tree_fn, self.spec, self.ranks, self.tables, self.chunk = tree_fn, spec, ranks, tables, int(chunk)
         self.n_threads = n_threads
+        self.dcfr_params, self.pcfr_gamma = dcfr_params, pcfr_gamma
         self.n_boards = spec.boards.shape[0]
         self.L = cfr2_c.lib()
         self.trunk_ft = tree_fn(spec_slice(spec, 0, 1))
@@ -162,7 +182,8 @@ class ChunkedOracle:
         nb = ft.board_spec.boards.shape[0]
         rk = np.full((nb + 1, ft.R), -1, np.int32)  # global board 0 is the empty pre-deal board
         rk[1:] = self.ranks[lo:lo + nb]
-        return cfr2_c.Oracle2CSolver(ft, rk, algo, delay=delay, n_threads=self.n_threads, lean=True)
+        return cfr2_c.Oracle2CSolver(ft, rk, algo, delay=delay, n_threads=self.n_threads, lean=True,
+                                     dcfr_params=self.dcfr_params, pcfr_gamma=self.pcfr_gamma)
 
     def chunks(self):
         for lo in range(0, self.n_boards, self.chunk):
@@ -170,13 +191,21 @@ class ChunkedOracle:
             yield lo, hi, self.tree_fn(spec_slice(self.spec, lo, hi))
 
     def _set(self, o, ft, lo, key):
-        o.regret[:], o.avg[:] = self.tables(ft, lo, key)
+        """the tables of `key` into solver o; strategy = regret matching of the regrets (PCFR+ solver: of the predictions)"""
+        tabs = self.tables(ft, lo, key)
+        o.regret[:], o.avg[:] = tabs[:2]
+        if o.pred is not None:
+            o.pred[:] = tabs[2]
         self.L.orc2_regret_match(C.byref(o.t))
+
+    def _factors(self, o, algo, it):
+        cfr2_c.set_factors(o.t, algo, it, self.dcfr_params, self.pcfr_gamma)
 
     # ------------------------------------------------------------------------------------------------ evaluation
     def evaluate(self, key, algo="CFRPlus", forms=("current", "average")):
         """Both seats' ev / ev_br at the chance node, and the exploitability, of the current strategy (regret matching of
-        the regrets) and of the average strategy (CFR+: the average rows; Vanilla / Linear CFR: the normalised sums).
+        the regrets; PCFR+: of the predictions) and of the average strategy (CFR+: the average rows; the others: the
+        normalised sums).
         Also abs_ev / abs_br: sum over the suit permutations s and boards b of |mult_b v_b[perm_s(h)]| (error bounds)."""
         R = self.trunk_ft.R
         acc = {f: {k: np.zeros((2, R)) for k in ("ev", "ev_br", "abs_ev", "abs_br")} for f in forms}
@@ -225,18 +254,28 @@ class ChunkedOracle:
         return t
 
     # ------------------------------------------------------------------------------------------------ half-iteration
-    def half_iterations(self, p, runs, on_chunk, chance_ev=None):
+    def half_iterations(self, p, runs, on_chunk, chance_ev=None, pending=False):
         """Seat p's half-iteration (_CFRBase.py:123-128) from the given tables, for every run (key, algo, iteration, delay).
-        The runs share one value sweep per chunk, so they must share the regrets.  on_chunk(lo, hi, ft, run index, regret,
-        avg) receives each chunk's post-update tables (float64 [ft.n_slots, R]; the trunk rows are the game's).  chance_ev:
-        seat p's chance-node row under the given strategy if known (evaluate()['current']['ev'][p]), else one more pass.
-        Returns per run the updated trunk rows: dict(regret, strat, avg [n_trunk_slots, R], reach [n_trunk_nodes, 2, R])."""
+        The runs share one value sweep per chunk, so they must share the strategy: the regrets (CFR+, Vanilla / Linear CFR
+        and DCFR runs together), or the predictions (PCFR+ runs only).  on_chunk(lo, hi, ft, run index, regret, avg[,
+        pred]) receives each chunk's post-update tables (float64 [ft.n_slots, R]; the trunk rows are the game's; pred for
+        PCFR+).  chance_ev: seat p's chance-node row under the given strategy if known (evaluate()['current']['ev'][p]),
+        else one more pass.  pending (p = 1, averages kept as sums): seat 0's average contribution of the same iteration
+        is added to the post-deal rows first, under the given profile (the deferred form of the board engine, whose trunk
+        rows already hold it: the trunk's are left alone).
+        Returns per run the updated trunk rows: dict(regret, strat, avg[, pred] [n_trunk_slots, R], reach [n_trunk_nodes,
+        2, R])."""
         ch, nts = self.chance_node, self.nts
-        key0 = runs[0][0]
+        key0, algo0 = runs[0][0], runs[0][1]
+        pcfr = algo0 == "PCFRPlus"
+        if any((algo == "PCFRPlus") != pcfr for _, algo, _, _ in runs):
+            raise ValueError("PCFR+ runs (strategies from the predictions) need a pass of their own")
+        if pending and (p != 1 or any(algo == "CFRPlus" for _, algo, _, _ in runs)):
+            raise ValueError("pending: seat 0's contribution to sums, before seat 1's update")
         if chance_ev is None:
             chance_ev = np.zeros(self.trunk_ft.R)
             for lo, hi, ft in self.chunks():
-                o = self._solver(ft, lo)
+                o = self._solver(ft, lo, algo0)
                 self._set(o, ft, lo, key0)
                 self.L.orc2_reach(C.byref(o.t), o.strat.ctypes.data)
                 self.L.orc2_values(C.byref(o.t), o.strat.ctypes.data, 1 << p, 0)
@@ -249,26 +288,33 @@ class ChunkedOracle:
             self.L.orc2_reach(tt, t.strat.ctypes.data)
             t.ev[ch, p] = chance_ev
             self.L.orc2_values_levels(tt, t.strat.ctypes.data, 1 << p, 0, self.chance_level, 1)
+            self._factors(t, algo, it)
             self.L.orc2_regret_update(tt, p, cfr2_c.ALGOS[algo], it)
             self.L.orc2_reach(tt, t.strat.ctypes.data)
             self.L.orc2_avg_update(tt, p, cfr2_c.ALGOS[algo], it, t.delay)
             trunk.append(dict(regret=t.regret[:nts].copy(), strat=t.strat[:nts].copy(), avg=t.avg[:nts].copy(),
-                              reach=t.reach[:self.n_trunk_nodes].copy()))
+                              reach=t.reach[:self.n_trunk_nodes].copy(), **({"pred": t.pred[:nts].copy()} if pcfr else {})))
             del t
         for lo, hi, ft in self.chunks():
-            o = self._solver(ft, lo)
+            o = self._solver(ft, lo, algo0)
             tt = C.byref(o.t)
             for k, (key, algo, it, delay) in enumerate(runs):
                 self._set(o, ft, lo, key)
+                self._factors(o, algo, it)
                 if k == 0:
                     self.L.orc2_reach(tt, o.strat.ctypes.data)
                     self.L.orc2_values(tt, o.strat.ctypes.data, 1 << p, 0)
+                if pending:  # seat 0's contribution under the given profile; its trunk rows are replaced below
+                    self.L.orc2_reach(tt, o.strat.ctypes.data)
+                    self.L.orc2_avg_update(tt, 0, cfr2_c.ALGOS[algo], it, 0)
                 self.L.orc2_regret_update(tt, p, cfr2_c.ALGOS[algo], it)
                 # the chunk's trunk rows above came from its own share of the chance node: the game's go in their place
                 o.regret[:nts], o.strat[:nts] = trunk[k]["regret"], trunk[k]["strat"]
+                if pcfr:
+                    o.pred[:nts] = trunk[k]["pred"]
                 self.L.orc2_reach(tt, o.strat.ctypes.data)
                 self.L.orc2_avg_update(tt, p, cfr2_c.ALGOS[algo], it, delay if algo == "CFRPlus" else 0)
                 o.avg[:nts] = trunk[k]["avg"]
-                on_chunk(lo, hi, ft, k, o.regret, o.avg)
+                on_chunk(lo, hi, ft, k, o.regret, o.avg, *((o.pred,) if pcfr else ()))
             del o
         return trunk

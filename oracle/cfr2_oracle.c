@@ -10,6 +10,11 @@
  *     lib_hand_eval.so (oracle/gen_golden_twocard.py), and
  *   - on whole sweeps / iterations against oracle/cfr2_numpy.py (dense sign matrices), which reproduces the reference's
  *     one-card values in the one-card limit (tests/test_oracle_cfr2.py).
+ * DCFR and PCFR+ (no reference implementation) are pinned at 1e-12 against their numpy restatements on cfr2_numpy's tree
+ * (tests/dcfr_common.Oracle2DCFR, tests/pcfr_common.Oracle2PCFR; tests/test_oracle_cfr2_c.py), with the caller's float32
+ * factors.  Run a chunk of boards at a time (oracle/cfr2_chunked.py, itself pinned against this file in one piece by
+ * tests/test_oracle_cfr2_chunked.py), it is the float64 side of the full-game board engine tests: CFR+ and Linear CFR
+ * (tests/test_gpu_board_full_game.py), DCFR and PCFR+ (tests/test_gpu_board_full_game_dcfr_pcfr.py).
  *
  * Same statements as oracle/cfr2_numpy.py, level by level over the flat tree (reach StrategyFiller.py:118-146, 148-169;
  * values + BR ValueFiller.py:21-101; regrets _CFRBase.py:146-185 with CFRPlus.py:37-41 / LinearCFR.py:27-31 /
@@ -30,7 +35,7 @@
 #endif
 
 enum { K_P0 = 0, K_P1 = 1, K_CHANCE = 2, K_FOLD = 3, K_SHOWDOWN = 4, K_SHOWDOWN_ALLIN = 5 };
-enum { ALGO_VANILLA = 0, ALGO_CFR_PLUS = 1, ALGO_LINEAR = 2 };
+enum { ALGO_VANILLA = 0, ALGO_CFR_PLUS = 1, ALGO_LINEAR = 2, ALGO_DCFR = 3, ALGO_PCFR_PLUS = 4 };
 
 typedef struct {
     int32_t n_nodes, n_levels, n_slots, R, n_deck, n_boards, n_sym, pad;
@@ -57,7 +62,10 @@ typedef struct {
     double* ev_br;
     double* regret; /* [n_slots][R] */
     double* strat;
-    double* avg;    /* CFR+: average strategy; Vanilla / Linear: reach-weighted sums */
+    double* avg;    /* CFR+: average strategy; Vanilla / Linear / DCFR / PCFR+: reach-weighted sums */
+    /* appended fields (the offsets above stay put) */
+    double* pred;   /* [n_slots][R] PCFR+: the predicted regrets Q = max(R + d, 0); NULL for the other algorithms */
+    double fa, fb, fw; /* factors of the next update: DCFR {a_t, b_t, w_t}, PCFR+ w_t (fw); set by the caller */
 } orc2_t;
 
 int orc2_set_threads(int n) {
@@ -288,8 +296,8 @@ void orc2_values(orc2_t* t, const double* strat, int mask, int with_br) {
     orc2_values_levels(t, strat, mask, with_br, t->n_levels - 1, 0);
 }
 
-/* strategy = regret matching of the stored regrets at every decision node (CFRPlus.py:43-63) */
-void orc2_regret_match(orc2_t* t) {
+/* strategy = regret matching of the rows `src` ([n_slots][R]) at every decision node (CFRPlus.py:43-63) */
+void orc2_match(orc2_t* t, const double* src) {
     const int R = t->R;
 #pragma omp parallel for schedule(dynamic, 64)
     for (int n = 0; n < t->n_nodes; ++n) {
@@ -297,14 +305,17 @@ void orc2_regret_match(orc2_t* t) {
         const int A = t->n_children[n], fs = t->slot[t->first_child[n]];
         for (int h = 0; h < R; ++h) {
             double s = 0.0;
-            for (int a = 0; a < A; ++a) s += fmax(t->regret[(size_t)(fs + a) * R + h], 0.0);
+            for (int a = 0; a < A; ++a) s += fmax(src[(size_t)(fs + a) * R + h], 0.0);
             for (int a = 0; a < A; ++a) {
-                const double r = fmax(t->regret[(size_t)(fs + a) * R + h], 0.0);
+                const double r = fmax(src[(size_t)(fs + a) * R + h], 0.0);
                 t->strat[(size_t)(fs + a) * R + h] = (s > 0.0) ? r / s : 1.0 / (double)A;
             }
         }
     }
 }
+
+/* strategy = regret matching of the stored regrets (PCFR+: of the stored predictions) */
+void orc2_regret_match(orc2_t* t) { orc2_match(t, t->pred ? t->pred : t->regret); }
 
 /* root exploitability per seat (ValueFiller.py:95-101) */
 void orc2_exploitability(const orc2_t* t, double* out) {
@@ -315,9 +326,48 @@ void orc2_exploitability(const orc2_t* t, double* out) {
     }
 }
 
+/* DCFR (Brown & Sandholm 2019) and PCFR+ (Farina, Kroer & Sandholm 2021) updates at seat p's nodes, with the caller's
+ * factors t->fa, t->fb (float32 values of pokerrl_b200.dcfr.factors, as the kernels read them):
+ *   DCFR:  x = d + R, R = x * (x > 0 ? a_t : b_t), strategy = matching of R
+ *   PCFR+: R = max(d + R, 0), Q = max(R + d, 0), strategy = matching of Q */
+static void regret_update_dp(orc2_t* t, int p, int algo) {
+    const int R = t->R;
+    const double fa = t->fa, fb = t->fb;
+#pragma omp parallel for schedule(dynamic, 64)
+    for (int n = 0; n < t->n_nodes; ++n) {
+        if (t->kind[n] != p || t->n_children[n] == 0) continue;
+        const int A = t->n_children[n], fc = t->first_child[n], fs = t->slot[fc];
+        const double* evn = ROW(t->ev, n, p);
+        double* src = (algo == ALGO_PCFR_PLUS) ? t->pred : t->regret;
+        for (int h = 0; h < R; ++h) {
+            double s = 0.0;
+            for (int a = 0; a < A; ++a) {
+                const double dlt = ROW(t->ev, fc + a, p)[h] - evn[h];
+                const size_t i = (size_t)(fs + a) * R + h;
+                if (algo == ALGO_PCFR_PLUS) {
+                    t->regret[i] = fmax(dlt + t->regret[i], 0.0);
+                    t->pred[i] = fmax(t->regret[i] + dlt, 0.0);
+                } else {
+                    const double x = dlt + t->regret[i];
+                    t->regret[i] = x * (x > 0.0 ? fa : fb);
+                }
+                s += fmax(src[i], 0.0);
+            }
+            for (int a = 0; a < A; ++a) {
+                const double r = fmax(src[(size_t)(fs + a) * R + h], 0.0);
+                t->strat[(size_t)(fs + a) * R + h] = (s > 0.0) ? r / s : 1.0 / (double)A;
+            }
+        }
+    }
+}
+
 /* regret update + regret matching at seat p's nodes (needs ev under the pre-update profile) */
 void orc2_regret_update(orc2_t* t, int p, int algo, int iter) {
     const int R = t->R;
+    if (algo == ALGO_DCFR || algo == ALGO_PCFR_PLUS) {
+        regret_update_dp(t, p, algo);
+        return;
+    }
 #pragma omp parallel for schedule(dynamic, 64)
     for (int n = 0; n < t->n_nodes; ++n) {
         if (t->kind[n] != p || t->n_children[n] == 0) continue;
@@ -343,9 +393,25 @@ void orc2_regret_update(orc2_t* t, int p, int algo, int iter) {
     }
 }
 
-/* average-strategy update of seat p's nodes (reach must be current under the new strategy) */
+/* average-strategy update of seat p's nodes (reach must be current under the new strategy); DCFR / PCFR+ weigh the
+ * contribution by the caller's w_t (t->fw) */
 void orc2_avg_update(orc2_t* t, int p, int algo, int iter, int delay) {
     const int R = t->R;
+    if (algo == ALGO_DCFR || algo == ALGO_PCFR_PLUS) {
+        const double w = t->fw;
+#pragma omp parallel for schedule(dynamic, 64)
+        for (int n = 0; n < t->n_nodes; ++n) {
+            if (t->kind[n] != p || t->n_children[n] == 0) continue;
+            const int A = t->n_children[n], fs = t->slot[t->first_child[n]];
+            const double* rp = ROW(t->reach, n, p);
+            for (int a = 0; a < A; ++a) {
+                double* av = t->avg + (size_t)(fs + a) * R;
+                const double* s = t->strat + (size_t)(fs + a) * R;
+                for (int h = 0; h < R; ++h) av[h] += s[h] * rp[h] * w;
+            }
+        }
+        return;
+    }
     double m_old = 0.0, m_new = 1.0;
     if (algo == ALGO_CFR_PLUS && iter > delay) { /* CFRPlus.py:68-73 */
         const double cw = 0.5 * ((double)iter * (iter + 1) - (double)delay * (delay + 1));
@@ -370,7 +436,8 @@ void orc2_avg_update(orc2_t* t, int p, int algo, int iter, int delay) {
     }
 }
 
-/* out[slot][h] = normalised average strategy (LinearCFR.py:64-71: uniform where the sum is 0); CFR+: copy of avg */
+/* out[slot][h] = normalised average strategy (LinearCFR.py:64-71: uniform where the sum is 0; Vanilla, Linear CFR, DCFR and
+ * PCFR+); CFR+: copy of avg */
 void orc2_average_strategy(const orc2_t* t, int algo, double* out) {
     const int R = t->R;
     if (algo == ALGO_CFR_PLUS) {

@@ -1,5 +1,6 @@
 """oracle/cfr2_oracle.c (float64, O(R) sorted-sweep showdowns, OpenMP) against oracle/cfr2_numpy.py (dense sign
-matrices) on whole sweeps and CFR iterations - two independent formulations of the same statements."""
+matrices) on whole sweeps and CFR iterations - two independent formulations of the same statements.  DCFR and PCFR+
+against their numpy restatements on the same trees (tests/dcfr_common.py, tests/pcfr_common.py)."""
 import numpy as np
 import pytest
 
@@ -72,3 +73,33 @@ def test_multi_street_and_isomorphic_trees():
     b.iteration()
     x, y = a.exploitability_current(), b.exploitability_current()
     assert abs(x - y) <= 1e-10 * abs(x)
+
+
+@pytest.mark.parametrize("stack", [20000, 600])
+@pytest.mark.parametrize("algo", ["DCFR", "PCFRPlus"])
+def test_dcfr_and_pcfr_iterations_match_numpy_oracles(algo, stack):
+    """DCFR and PCFR+ iterations of the C oracle against the numpy restatements (tests/dcfr_common.py, tests/pcfr_common.py),
+    both seats' half-iterations at counters 0 .. 3 and at 997 (w_t about 1e6): values, regrets, predictions, sums and
+    both exploitabilities; both sides take the float32 factors of pokerrl_b200.dcfr"""
+    from dcfr_common import Oracle2DCFR
+    from pcfr_common import Oracle2PCFR
+    ft = fhp_tree(random_board_spec(6, 3), stack)
+    orc = oracle_tree(ft)
+    norm = ft.game_cls.EV_NORMALIZER
+    a = Oracle2DCFR(orc, ev_normalizer=norm) if algo == "DCFR" else Oracle2PCFR(orc, 2.0, ev_normalizer=norm)
+    b = cfr2_c.Oracle2CSolver(ft, orc.board_ranks, algo, n_threads=4)
+    for t in (0, 1, 2, 3, 997):
+        a.iter_counter = b.iter_counter = t
+        for p in (0, 1):
+            a.half_iteration(p)
+            b.half_iteration(p)
+            errs = [_rel(b.ev, a.t.ev), _rel(b.reach, a.t.reach), _rel(b.regret, a.regret), _rel(b.avg, a.avg)]
+            if algo == "PCFRPlus":
+                errs.append(_rel(b.pred, a.pred))
+                assert (b.regret >= 0).all() and (b.pred >= 0).all()
+            assert max(errs) <= 1e-12, (t, p, errs)
+        x, y = a.exploitability_current(), b.exploitability_current()
+        assert abs(x - y) <= 1e-12 * abs(x), (t, x, y)
+        x, y = a.exploitability_average(), b.exploitability_average()
+        assert abs(x - y) <= 1e-12 * abs(x), (t, x, y)
+        print("%s stack %d counter %d: relative errors %s" % (algo, stack, t, " ".join("%.1e" % e for e in errs)))
