@@ -32,8 +32,9 @@ typedef void* prl_stream_t; /* cudaStream_t */
     prl_board_layout / prl_board_rows / prl_board_policy_query take the shape; 8: PRL_ALGO_DCFR, prl_buffers_t / prl_board_game_t
     gained the DCFR factor table `dcfr`; 9: PRL_ALGO_PCFR_PLUS, which reads w_t from that table, prl_board_game_t gained the
     prediction table `pred`; 10: restricted Nash response, prl_board_game_t gained the model reach table `rnr_reach` and the
-    mixing probability `rnr_p`, prl_trunk_t the model's trunk reach `reach_model` and `rnr_p`) */
-#define PRL_ABI_VERSION 10
+    mixing probability `rnr_p`, prl_trunk_t the model's trunk reach `reach_model` and `rnr_p`; 11: prl_board_game_t gained the
+    best-response action table `br_out`) */
+#define PRL_ABI_VERSION 11
 
 /* node kinds (game/_/tree/_/nodes.py:8-62 + ValueFiller.py:34-62) */
 enum {
@@ -281,6 +282,8 @@ typedef struct {
                                 (the opponent of the sweep's seat) at the board's n_sd showdown terminals, strength order, deal
                                 probability and the model's trunk reach included; NULL: a plain sweep.  See prl_board_sweep. */
     float rnr_p;             /* probability of the model in the opponent's mixture, [0, 1] */
+    float* br_out;           /* DEVICE float[n_rows][ldb] laid out as `regret`: the evaluation sweep of seat p writes one-hot rows of
+                                p's best-response actions at p's decision nodes (NULL: nothing written).  See prl_board_sweep. */
 } prl_board_game_t;
 
 /* out[8] = {n_live, ldb, blob bytes per board, byte offset of the int16 hand ids, byte offset of the card rows,
@@ -314,7 +317,11 @@ int prl_board_build_tables(const int32_t* ranks, const uint64_t* board_mask, con
  * opponent's reach at the showdown terminals is the sweep's own (from trunk_reach_opp, which the caller scales by 1 - rnr_p)
  * plus rnr_p * rnr_reach, at the fold terminals the same combination through the fold identity.  The update (here or through
  * prl_board_update_cfrp) and the evaluation read rnr_reach; p1_only != 0 instead WRITES rnr_reach: the opponent's reach at the
- * showdown terminals under the rows of `avg` as they are (the model) and trunk_reach_opp (the model's), nothing else. */
+ * showdown terminals under the rows of `avg` as they are (the model) and trunk_reach_opp (the model's), nothing else.
+ * Best-response export (eval != 0, g->br_out != NULL, not with rnr_reach): at every decision node of seat p, for every live
+ * strength position, 1.0f on the row of the best-response child and 0.0f on the node's other rows; positions n_live .. ldb - 1
+ * of those rows are written as 0.  The best-response child is the FIRST child in child order whose ev_br equals the node's
+ * maximum (np.argmax over the children).  The opponent's rows of br_out are not touched. */
 int prl_board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, int src_opp, const float* trunk_reach_opp,
                     int iter, int delay, int algo, float defer_w, int p1_only, prl_stream_t stream);
 

@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("PRL_LIB_PATH") or os.path.join(_HERE, "lib", "libpoke
 # enums of include/pokerrl_b200.h
 KIND_P0, KIND_P1, KIND_CHANCE, KIND_FOLD, KIND_SHOWDOWN, KIND_SHOWDOWN_ALLIN = range(6)
 ALGO_VANILLA, ALGO_CFR_PLUS, ALGO_LINEAR, ALGO_DCFR, ALGO_PCFR_PLUS = 0, 1, 2, 3, 4
-ABI_VERSION = 10  # include/pokerrl_b200.h: PRL_ABI_VERSION
+ABI_VERSION = 11  # include/pokerrl_b200.h: PRL_ABI_VERSION
 STRAT_F32, STRAT_UNIFORM64, STRAT_AVG_F64, STRAT_AVG_SUM, STRAT_AVG_F32 = range(5)
 
 
@@ -51,7 +51,7 @@ class PrlBoardGame(C.Structure):
                 ("row0", C.c_int64 * 16), ("row_m", C.c_int32 * 16),
                 ("tables", C.c_void_p), ("board_prob", C.c_void_p), ("board_mult", C.c_void_p), ("regret", C.c_void_p),
                 ("avg", C.c_void_p), ("w_private", C.c_void_p), ("w_total", C.c_void_p), ("dcfr", C.c_void_p), ("pred", C.c_void_p),
-                ("rnr_reach", C.c_void_p), ("rnr_p", C.c_float)]
+                ("rnr_reach", C.c_void_p), ("rnr_p", C.c_float), ("br_out", C.c_void_p)]
 
 
 class PrlTrunk(C.Structure):

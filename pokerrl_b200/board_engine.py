@@ -908,6 +908,45 @@ class BoardPolicyEvaluator(_BoardEngine):
     def evaluate(self, agent, profile=False):
         """exploitability of each seat in chips, numpy float64 [2] (the analogue of PublicTree's root.exploitability).
         profile=True synchronises between the phases and leaves their wall times (s) in self.times."""
+        return self._evaluate(agent, profile)
+
+    def best_response(self, agent, profile=False):
+        """(exploitability, tables): evaluate(agent)'s numbers, bit for bit, and the best response to `agent` at both seats as a
+        BoardPolicyTables (seat s's rows = seat s's best response).  Each evaluation sweep writes one-hot rows of its seat's
+        best-response actions into one table over the whole spec (prl_board_sweep with br_out); the trunk's rows are one-hot
+        rows of the best-response values the trunk evaluation leaves in bufs.ev_br.  At every node the action is the FIRST
+        child in child order whose best-response value is the maximum (np.argmax; PublicTree's br_a_idx_in_child_arr_for_each_hand).
+        Raises ValueError before allocating when the table and its position -> hand rows do not fit in free device memory
+        (best_response_bytes: 8.19 GB + 291 MB for the 134 459 classes at stacks of 901 chips and more)."""
+        import hashlib
+        nb, rpb, L, dev = self.n_boards_total, self.rows_per_board, self.L, self.device
+        need = best_response_bytes(nb, rpb)
+        with torch.cuda.device(dev):
+            free, _ = torch.cuda.mem_get_info(dev)
+            check_best_response_fits(need, free + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev))
+            rows = torch.empty((nb * rpb, L["ldb"]), dtype=torch.float32, device=dev)
+            pos_hand = torch.empty((nb, L["n_live"]), dtype=torch.int16, device=dev)
+            e = self._evaluate(agent, profile, rows, pos_hand)
+            ft, nts, R = self.ft1, self.n_trunk_slots, self.R
+            trunk = torch.zeros((nts, self.ld), dtype=torch.float32, device=dev)
+            for n in range(self.chance_node + 1):
+                if ft.kind[n] <= 1 and ft.first_child[n] >= 0:
+                    fs, fc, A = int(ft.first_slot[n]), int(ft.first_child[n]), int(ft.n_children[n])
+                    trunk[fs:fs + A, :R] = first_max_onehot(self.bufs.ev_br[int(ft.kind[n]), fc:fc + A, :R], 0)
+            keys = board_keys(self.spec.boards)
+            if np.any(np.diff(keys) <= 0):  # rows by ascending key, as BoardPolicyTables.from_solver
+                perm = np.argsort(keys, kind="stable")
+                t_perm = torch.from_numpy(perm).to(dev)
+                rows = rows.view(nb, rpb, -1)[t_perm].reshape(nb * rpb, -1)
+                pos_hand = pos_hand[t_perm]
+                keys = keys[perm]
+            t_keys = torch.from_numpy(keys).to(dev)
+        spec_id = (int(nb), self.n_sym > 0, hashlib.sha1(keys.tobytes()).hexdigest())
+        return e, BoardPolicyTables(rows, t_keys, pos_hand, trunk, self.n_sym > 0, _packed_actions(self.ft1, self.st),
+                                    abstract_fingerprint(self.ft1), spec_id)
+
+    def _evaluate(self, agent, profile, br_rows=None, pos_hand=None):
+        """evaluate(); br_rows / pos_hand (best_response): the tables the sweeps export into, over the whole spec"""
         import time
         dev = self.device
         times = {"agent query": 0.0, "table build": 0.0, "sweeps": 0.0}
@@ -923,11 +962,18 @@ class BoardPolicyEvaluator(_BoardEngine):
 
         with torch.cuda.device(dev):
             self.w_acc.zero_()
-            for lo, hi, t0 in self._chunks(agent, tick):
-                for p in (0, 1):  # prl_board_sweep zeroes the arrays it writes at every launch: accumulate outside
-                    self._board_sweep(self.bufs, p, True, SRC_AVG, SRC_AVG, 0, 0, nat.ALGO_CFR_PLUS)
-                    self.w_acc[2 * p:2 * p + 2] += self.w_total[2 * p:2 * p + 2]
-                tick("sweeps", t0)
+            try:
+                for lo, hi, t0 in self._chunks(agent, tick):
+                    if br_rows is not None:
+                        self.g.br_out = br_rows[lo * self.rows_per_board].data_ptr()
+                        sh = self.L["sh_off"]
+                        pos_hand[lo:hi] = self.t_blob[:hi - lo, sh:sh + 2 * self.L["n_live"]].contiguous().view(torch.int16)
+                    for p in (0, 1):  # prl_board_sweep zeroes the arrays it writes at every launch: accumulate outside
+                        self._board_sweep(self.bufs, p, True, SRC_AVG, SRC_AVG, 0, 0, nat.ALGO_CFR_PLUS)
+                        self.w_acc[2 * p:2 * p + 2] += self.w_total[2 * p:2 * p + 2]
+                    tick("sweeps", t0)
+            finally:
+                self.g.br_out = None
             t0 = time.perf_counter()
             self.w_total.copy_(self.w_acc)
             self._board_trunk(self.bufs, modes, True, -1, 0, 0, nat.ALGO_CFR_PLUS)
@@ -935,6 +981,31 @@ class BoardPolicyEvaluator(_BoardEngine):
             tick("sweeps", t0)
         self.times = times
         return e
+
+
+def best_response_bytes(n_boards, rows_per_board):
+    """device bytes of BoardPolicyEvaluator.best_response's tables: the strength-ordered rows (1088 floats per row) and the
+    int16 position -> hand rows (1081 per board)"""
+    return n_boards * rows_per_board * 1088 * 4 + n_boards * 1081 * 2
+
+
+def check_best_response_fits(need, free):
+    """ValueError, with the byte counts, when `need` bytes of best-response tables exceed `free` device bytes"""
+    if need > free:
+        raise ValueError("the best-response tables of this spec need %d bytes (%.2f GB) of device memory, %d bytes (%.2f GB) "
+                         "are free" % (need, need / 1e9, free, free / 1e9))
+
+
+def first_max_onehot(v, dim):
+    """float32 one-hot of the FIRST index along `dim` whose entry equals the maximum (np.argmax's rule), same shape as v"""
+    m = v.amax(dim=dim, keepdim=True)
+    n = v.shape[dim]
+    idx = torch.zeros_like(m, dtype=torch.int64)
+    for c in reversed(range(n)):
+        idx = torch.where(v.narrow(dim, c, 1) == m, c, idx)
+    shape = [1] * v.dim()
+    shape[dim] = n
+    return (torch.arange(n, device=v.device).view(shape) == idx).to(torch.float32)
 
 
 class BoardPolicyTables:

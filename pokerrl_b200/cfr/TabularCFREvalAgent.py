@@ -65,10 +65,16 @@ class TabularCFREvalAgent(EvalAgentBase):
         solver = cfr.solvers[tree_idx]
         if getattr(solver, "ft", None) is None and hasattr(solver, "ft1"):  # board engine: no slot table
             from pokerrl_b200.board_engine import BoardPolicyTables
-            agent._board = BoardPolicyTables.from_solver(solver)
-            agent._fingerprint = (agent._board.fingerprint, agent._board.spec_id)
-            return agent
+            return cls.from_board_tables(t_prof, BoardPolicyTables.from_solver(solver))
         agent.update_weights((average_strategy_table(solver), tree_fingerprint(solver.ft)))
+        return agent
+
+    @classmethod
+    def from_board_tables(cls, t_prof, tables):
+        """the agent that plays a board_engine.BoardPolicyTables (a board-engine solver's average, a best response)"""
+        agent = cls(t_prof=t_prof)
+        agent._board = tables
+        agent._fingerprint = (tables.fingerprint, tables.spec_id)
         return agent
 
     def can_compute_mode(self):

@@ -326,12 +326,18 @@ __device__ __forceinline__ void st_stream(float* p, float v) { __stcs(p, v); }
 // holds for any opponent whose rows sum to one.  CFR+ update forms (the exploiter's update) and the evaluation form (the
 // exploitation of the model, with rnr_p = 1 and a zero trunk_reach_opp).  kRnrOut: P1 only, the opponent's strategy = the rows
 // of `avg` as they are (the model), its showdown reach written to G.rnr_reach instead of S.
+// BREX (evaluation form): the best response is exported as well - at each of seat P's decision nodes P3 writes, per strength
+// position, 1.0f to the G.br_out row of the FIRST child whose br equals the node's maximum (np.argmax's rule; the maximum is
+// the fmaxf chain the value backup takes anyway) and 0.0f to the node's other rows; the padding positions kLive .. kLdb - 1 of
+// P's rows are written as 0.  The opponent's rows of G.br_out are never touched.
 constexpr int kRnrMix = 1, kRnrOut = 2;
-template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true, bool PRED = false, int RNR = 0>
+template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true, bool PRED = false, int RNR = 0,
+          bool BREX = false>
 __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArgs a) {
     static_assert(!(EVAL && DEFER) && (!P1ONLY || DEFER || RNR == kRnrOut) && (AVG || (!EVAL && !DEFER)), "variants");
     static_assert(!PRED || (DEFER && !P1ONLY), "PRED is an update form of the DEFER family");
     static_assert(RNR == 0 || (!DEFER && !PRED && (RNR == kRnrOut) == P1ONLY && (RNR == kRnrMix || !EVAL)), "RNR forms");
+    static_assert(!BREX || (EVAL && RNR == 0), "BREX is an export of the plain evaluation form");
     using M = SweepSmem<SH>;
     constexpr int NSD = SH::n_sd, NF = SH::n_fold;
     extern __shared__ __align__(128) unsigned char smem[];
@@ -791,6 +797,16 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
 #pragma unroll
                             for (int c = 1; c < A; ++c) b = fmaxf(b, br[fc + c]);
                             br[n] = b;
+                            if constexpr (BREX) {  // one-hot rows of the first child whose br is the maximum
+                                float* xrow = G.br_out + (size_t)j * kBoardFloats + (size_t)SH::row_of(fc) * kLdb + i;
+                                bool found = false;
+#pragma unroll
+                                for (int c = 0; c < A; ++c) {
+                                    const bool pick = !found && br[fc + c] == b;
+                                    found = found || pick;
+                                    st_stream(xrow + (size_t)c * kLdb, pick ? 1.0f : 0.0f);
+                                }
+                            }
                         } else {
                             if constexpr (PRED) {  // PCFR+: R = max(d + R, 0) (CFRPlus.py:37-41), then Q = max(R + d, 0)
 #pragma unroll
@@ -835,6 +851,11 @@ __global__ void __launch_bounds__(kThreads, 2) board_sweep_kernel(const SweepArg
         p3_load(2, gA, aA);
         if (p3_pos(1) < kLive) p3_hand(1, gB, aB);
         if (p3_pos(2) < kLive) p3_hand(2, gA, aA);
+        if constexpr (BREX) {  // the padding positions of the seat's exported rows
+            if (tid < kLdb - kLive)
+#pragma unroll
+                for (int r = 0; r < NOWN; ++r) st_stream(G.br_out + (size_t)j * kBoardFloats + (size_t)(OWN0 + r) * kLdb + kLive + tid, 0.0f);
+        }
         }  // !P1ONLY
         // next unit's P1 inputs: requested before the barrier below, consumed after it (the other table buffer is long there)
         if (jn < nb) {
@@ -1360,9 +1381,10 @@ int default_grid() {
     return cached[dev];
 }
 
-template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true, bool PRED = false, int RNR = 0>
+template <class SH, int P, bool EVAL, bool DEFER = false, bool P1ONLY = false, bool AVG = true, bool PRED = false, int RNR = 0,
+          bool BREX = false>
 int launch_sweep(const SweepArgs& a, int grid, cudaStream_t s) {
-    auto kern = board_sweep_kernel<SH, P, EVAL, DEFER, P1ONLY, AVG, PRED, RNR>;
+    auto kern = board_sweep_kernel<SH, P, EVAL, DEFER, P1ONLY, AVG, PRED, RNR, BREX>;
     constexpr int kSmemBytes = SweepSmem<SH>::kSmemBytes;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);  // per device: set every time
     if (e != cudaSuccess) return prl::check(e, "prl_board_sweep: shared memory opt-in");
@@ -1425,6 +1447,9 @@ static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, 
     const bool rnr = g->rnr_reach != nullptr;
     if (rnr && algo != PRL_ALGO_CFR_PLUS) return prl::fail("prl_board_sweep: the restricted Nash response is a CFR+ form");
     if (rnr && !(g->rnr_p >= 0.0f && g->rnr_p <= 1.0f)) return prl::fail("prl_board_sweep: rnr_p must be in [0, 1]");
+    const bool brex = g->br_out != nullptr;
+    if (brex && (!eval || p1_only || rnr))
+        return prl::fail("prl_board_sweep: br_out is written by the evaluation sweep without a restricted Nash response only");
     if (p1_only && !defer && !rnr)
         return prl::fail("prl_board_sweep: p1_only is the average flush of Vanilla / Linear CFR or the model reach of a restricted "
                          "Nash response");
@@ -1479,6 +1504,8 @@ static int board_sweep(const prl_board_game_t* g, int p, int eval, int src_own, 
         using SH = decltype(sh);
         if (eval && rnr) return (p == 0) ? launch_sweep<SH, 0, true, false, false, true, false, kRnrMix>(a, grid, s)
                                          : launch_sweep<SH, 1, true, false, false, true, false, kRnrMix>(a, grid, s);
+        if (eval && brex) return (p == 0) ? launch_sweep<SH, 0, true, false, false, true, false, 0, true>(a, grid, s)
+                                          : launch_sweep<SH, 1, true, false, false, true, false, 0, true>(a, grid, s);
         if (eval) return (p == 0) ? launch_sweep<SH, 0, true>(a, grid, s) : launch_sweep<SH, 1, true>(a, grid, s);
         if (rnr && step) return (p == 0) ? launch_sweep<SH, 0, false, false, false, true, false, kRnrMix>(a, grid, s)
                                          : launch_sweep<SH, 1, false, false, false, true, false, kRnrMix>(a, grid, s);

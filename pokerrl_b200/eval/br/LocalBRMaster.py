@@ -59,6 +59,25 @@ class LocalBRMaster(EvaluatorMasterBase):
     def update_weights(self):
         self._eval_agent.update_weights(copy.deepcopy(self.pull_current_strat_from_chief()))
 
+    def best_response_agent(self, stack_size_idx=0):
+        """(e0, e1, agent): the exploitability of each seat of the current eval agent at evaluation stack stack_size_idx, in the
+        game's metric (the numbers evaluate() logs the mean of), and its best response as a TabularCFREvalAgent - seat s's rows
+        are seat s's best response.  At every node the action is the FIRST child in child order whose best-response value is
+        the maximum (np.argmax).  Board engine: the agent holds the BoardPolicyTables of BoardPolicyEvaluator.best_response
+        (for the full Flop5Holdem game about 8.5 GB of device memory besides the evaluated agent's); level engine: the
+        one-hot slot table of PublicTree.best_response_table with the tree's fingerprint."""
+        from pokerrl_b200.cfr.TabularCFREvalAgent import TabularCFREvalAgent, tree_fingerprint
+        gt = self._game_trees[stack_size_idx]
+        norm = self._env_bldr.env_cls.EV_NORMALIZER
+        self._eval_agent.set_stack_size(stack_size=self._t_prof.eval_stack_sizes[stack_size_idx])
+        if not isinstance(gt, PublicTree):  # board engine
+            e, tables = gt.best_response(self._eval_agent)
+            return float(e[0]) * norm, float(e[1]) * norm, TabularCFREvalAgent.from_board_tables(self._t_prof, tables)
+        e0, e1 = self._compute_br_heads_up(stack_size_idx=stack_size_idx)
+        agent = TabularCFREvalAgent(t_prof=self._t_prof)
+        agent.update_weights((gt.best_response_table().cpu().numpy(), tree_fingerprint(gt.flat)))
+        return e0, e1, agent
+
     def _compute_br_heads_up(self, stack_size_idx, iter_nr=None, do_export_tree=True):
         gt = self._game_trees[stack_size_idx]
         norm = self._env_bldr.env_cls.EV_NORMALIZER

@@ -308,6 +308,29 @@ class PublicTree:
         self._cache.pop("ev", None)
         self._cache.pop("ev_br", None)
 
+    def best_response_table(self):
+        """after compute_ev: float32 [n_slots, R] on the tree's device, one-hot rows of the best response of the seat acting at
+        each decision node - 1 on the FIRST child in child order whose ev_br is the maximum, the child
+        br_a_idx_in_child_arr_for_each_hand names"""
+        from pokerrl_b200.board_engine import first_max_onehot
+        assert self._has_ev, "compute_ev() first"
+        ft, dev, R = self.flat, self.dtree.device, self.flat.R
+        dec = self.decision_nodes()
+        n_ch = ft.n_children[dec].astype(np.int64)
+        a_max = int(n_ch.max())
+        k = np.arange(a_max)
+        valid = k[None, :] < n_ch[:, None]
+        child = np.where(valid, ft.first_child[dec][:, None] + k[None, :], 0)
+        seat = np.broadcast_to(ft.kind[dec].astype(np.int64)[:, None], child.shape)
+        t_valid = torch.from_numpy(valid).to(dev)
+        v = self.bufs.ev_br[torch.from_numpy(seat).to(dev), torch.from_numpy(child).to(dev), :R]  # [n_dec, a_max, R]
+        v = torch.where(t_valid[:, :, None], v, torch.full_like(v, -float("inf")))
+        onehot = first_max_onehot(v, 1)
+        out = torch.zeros((ft.n_slots, R), dtype=torch.float32, device=dev)
+        slots = ft.first_slot[dec][:, None] + k[None, :]
+        out[torch.from_numpy(slots[valid]).to(dev)] = onehot[t_valid]
+        return out
+
     # ---- host access
     def _host(self, name):
         if name not in self._cache:
